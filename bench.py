@@ -1,9 +1,10 @@
 #!/usr/bin/env python
 """bench.py -- megapixels/sec of the USDU tile path (BASELINE.json: "megapixels/sec 4K->8K
-SDXL tile-upscale at 1/2/4/8 B200; blend HBM GB/s").
+SDXL tile-upscale at 1/2/4/8 H100; blend HBM GB/s").
 
   python bench.py --gpus N --steps K --warmup W              our arm (CUDA kernels)
   python bench.py --impl reference --gpus N --steps K ...    the reference's CPU path (port)
+  python bench.py ... --dump-outputs DIR                     also write the last timed step's result to DIR/*.npy
 
 A step is one full pass of the hot path over one synthetic canvas: quantise -> per wave
 (crop+LANCZOS kernel, sampler call, LANCZOS-back+composite kernel) -> dequantise.
@@ -128,7 +129,7 @@ def measured_peak_gbs():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.isfile(p):
         return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (NVIDIA H100 SXM data sheet: 3.35 TB/s HBM3)"
 
 
 def expected_digest(workload: str, world: int):
@@ -144,6 +145,40 @@ def expected_digest(workload: str, world: int):
         if f"{key}/{src}" in db:
             return db[f"{key}/{src}"], f"{key}/{src}"
     return None, key
+
+
+DUMP_SAMPLES = 1 << 21          # seeded random elements of the result: 8 MB as float32, their indices 16 MB as float64
+DUMP_GRID_BYTES = 32 << 20      # the strided grid: the smallest power-of-two stride >= 8 that keeps it within 32 MB
+
+
+def dump_outputs(out, directory: str) -> dict:
+    """Write the result [B,H,W,3] fp32 of a step as float32 .npy files: a fixed, seeded sample of its elements
+    (result_sample.npy, flat indices in result_sample_index.npy as float64), the strided grid out[:, ::s, ::s, :]
+    (result_strided.npy, s = 8 on the default workload) and the per-frame, per-channel sums in float64 (result_sums.npy)
+    -- at most 64 MB in all, and the same elements on every run with the same arguments, so two builds can be compared
+    output for output."""
+    import numpy as np
+    import torch
+    os.makedirs(directory, exist_ok=True)
+    flat = out.detach().reshape(-1)
+    n = flat.numel()
+    idx = np.sort(np.random.default_rng(0).choice(n, size=min(DUMP_SAMPLES, n), replace=False))
+    B, H, W, C = out.shape
+    stride = 8
+    while B * -(-H // stride) * -(-W // stride) * C * 4 > DUMP_GRID_BYTES:
+        stride *= 2
+    arrays = {
+        "result_sample": flat[torch.from_numpy(idx).to(flat.device)].to(torch.float32).cpu().numpy(),
+        "result_sample_index": idx.astype(np.float64),
+        "result_strided": out.detach()[:, ::stride, ::stride, :].to(torch.float32).cpu().numpy(),
+        "result_sums": out.detach().to(torch.float64).sum(dim=(1, 2)).cpu().numpy(),
+    }
+    total = sum(a.nbytes for a in arrays.values())
+    assert total <= 64 << 20, f"dump of {total} bytes exceeds 64 MB"
+    for name, a in arrays.items():
+        np.save(os.path.join(directory, f"{name}.npy"), np.ascontiguousarray(a))
+    return {"dir": directory, "files": sorted(f"{k}.npy" for k in arrays), "bytes": total, "shape": list(out.shape),
+            "stride": stride}
 
 
 def result_digest(out) -> str:
@@ -280,8 +315,8 @@ def cpu_baseline_sample(workload: str, n_tiles: int, budget_s: float):
 
 
 def run_reference(args):
-    """--impl reference: the reference's own CPU implementation of the path on the host cores, one bounded sample
-    (whatever --steps says: a sample is tens of seconds to minutes of CPU work).  N == 1: process_single_gpu.
+    """--impl reference: the reference's own CPU implementation of the path on the host cores, one bounded sample per
+    step (a sample is seconds to minutes of CPU work; the value is their mean).  N == 1: process_single_gpu.
     N > 1: the N-participant HTTP + PNG static mode.  Falls back to the cost-faithful port (oracle/ref_port*.py) only
     when oracle/_ref is missing."""
     rank = int(os.environ.get("RANK", "0"))
@@ -290,13 +325,11 @@ def run_reference(args):
     workload = args.workload
     B, H, W, tile, pad, blur = WORKLOADS[workload]
     mp = B * H * W / 1e6
-    steps = max(1, args.steps)
-    # every step is a bounded sample; the whole run stays within a few minutes whatever K is: the tiles of the sample are
-    # divided over the steps, and the loop stops taking new samples after 150 s (steps actually taken are reported)
-    vals, detail, t_start = [], None, time.perf_counter()
+    steps = args.steps
+    # exactly K steps, each one bounded sample; the tiles of the N = 1 sample are divided over the steps so that the run
+    # takes about as long whatever K is
+    vals, detail = [], None
     for i in range(steps):
-        if vals and time.perf_counter() - t_start > 150.0:
-            break
         if reference_available():
             if args.gpus == 1:
                 detail = real_reference_sample(workload, max(1, args.ref_tiles // steps))
@@ -329,7 +362,7 @@ def run_reference(args):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=10)
+    ap.add_argument("--steps", type=int, default=10, help="timed steps (--impl reference: bounded samples of the job)")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--workload", default="cfg2_4k_to_8k_sdxl_512px", choices=list(WORKLOADS))
@@ -344,7 +377,11 @@ def main():
     ap.add_argument("--semantics", default="static", choices=["static", "exact"],
                     help="N > 1: the reference's static mode (default, the headline) or the cooperative single-GPU DAG "
                          "(dist.upscale_exact: bit-identical to N = 1 at any world size; device-resident line only)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the result of the last one to DIR/*.npy (see dump_outputs)")
     args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
     if args.impl == "reference":
         return run_reference(args)
 
@@ -480,8 +517,15 @@ def main():
     stats = {}
     nvl = NvlinkCounters(local) if world > 1 else None
     nvl0 = nvl.read() if nvl else None
-    ms_step = timed(lambda: step_device(stats), args.steps)
+    last = []                                       # the result of the last timed step (a caller would receive it)
+
+    def step_kept():
+        last[:] = [step_device(stats)]
+
+    ms_step = timed(step_kept, args.steps)
     nvl1 = nvl.read() if nvl else None
+    dumped = dump_outputs(last[0], args.dump_outputs) if args.dump_outputs and rank == 0 else None
+    del last[:]
     nvlink = None
     if nvl0 is not None and nvl1 is not None:
         t = torch.tensor([(nvl1[0] - nvl0[0]) / args.steps, (nvl1[1] - nvl0[1]) / args.steps], dtype=torch.float64, device=dev)
@@ -494,13 +538,13 @@ def main():
         if rx0 > 0:
             nvlink["master_rx_GBps_if_spread_over_the_step"] = round(rx0 / (ms_step * 1e-3) / 1e9, 1)
     # (the sampler keeps running through the per-kernel and end-to-end timed loops below: K steps of a
-    # 1.3 ms job are over before nvidia-smi's first 100 ms tick)
+    # job of a few ms can be over before nvidia-smi's first 100 ms tick)
     stats["gpu_launches"] = stats.get("gpu_launches", 0) // args.steps        # per step
     stats["algo_bytes"] = stats.get("algo_bytes", 0) // args.steps
 
     # ---- per-kernel time of the dominant kernels, in situ -------------------------------------------
-    # N == 1: the wave loop is a CUDA graph; event-record nodes between its ~95 kernels cost ~0.5 ms per
-    # step (measured: 1.46 vs 2.01 ms), so the kernels are timed by DIFFERENCING instead: the same K
+    # N == 1: the wave loop is a CUDA graph; event-record nodes between its ~95 kernels would add a large
+    # share of the step they measure, so the kernels are timed by DIFFERENCING instead: the same K
     # steps with a graph that lacks the blend (resp. crop) launches; the difference is what the kernel
     # costs where it runs (launch latency and cache state included).  N > 1: CUDA events around every
     # launch (the final ordered blend is an eager launch there).
@@ -515,7 +559,7 @@ def main():
             wl_bytes["blend"] += plan.blend_worklist(w, offs_w, 4, None, B).algo_bytes * B
         # Kernel DURATIONS are taken in the plain level loop (schedule "waves": one kernel at a time).  The timed step above
         # runs the default schedule (split_crop), where the early crop jobs of level k+1 overlap blend(k): differencing THAT
-        # graph would credit the blend with the crop time it hides (measured: 12.7 instead of 14.8 us per launch).
+        # graph would credit the blend with the crop time it hides.
         timed_schedule = engine.SCHEDULE
         engine.SCHEDULE = "waves"
         try:
@@ -598,7 +642,7 @@ def main():
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     for _ in range(max(args.warmup, 3)):
         out_host = step_e2e()      # keep the result like the timed loop does: the second pinned result
-                                   # buffer (a one-time ~150 ms page-locking cost) is created here, not in the timed region
+                                   # buffer (a one-time page-locking cost) is created here, not in the timed region
     barrier()
     t0 = time.perf_counter()
     e0.record()
@@ -714,6 +758,8 @@ def main():
             "gpu_launches_per_step": stats.get("gpu_launches", 0),
             "parity": parity,
             "roofline": roofline}
+    if dumped is not None:
+        line["dump_outputs"] = dumped
     if phases is not None:
         line["phase_ms_max_over_ranks"] = phases
     if nvlink is not None:

@@ -1,4 +1,4 @@
-"""comfyui-distributed_b200 -- B200-native drop-in for the Ultimate-SD-Upscale tile hot
+"""comfyui-distributed_b200 -- H100-native drop-in for the Ultimate-SD-Upscale tile hot
 path of ComfyUI-Distributed (tile scatter -> per-tile denoise -> gather -> seam blend).
 
 ComfyUI loads this directory as a custom node package and reads NODE_CLASS_MAPPINGS

@@ -55,6 +55,7 @@ _SIGNATURES = {
     "usdu_abi_version": (c_int, []),
     "usdu_last_error": (c_char_p, []),
     "usdu_device_count": (c_int, []),
+    "usdu_sm_count": (c_int, []),
     "usdu_resample_ksize": (c_int, [c_int, c_int]),
     "usdu_resample_table_words": (c_int64, [c_int, c_int]),
     "usdu_build_resample_table": (c_int, [c_int, c_int, POINTER(c_int32)]),
@@ -132,6 +133,12 @@ def _i32p(a: np.ndarray):
 
 
 # ---- host-side builders -------------------------------------------------------------
+def sm_count() -> int:
+    """SMs of the current CUDA device (the count the launchers size their grids with), or 0 without a device."""
+    n = lib().usdu_sm_count()
+    return n if n > 0 else 0
+
+
 def build_resample_table(in_size: int, out_size: int) -> np.ndarray:
     L = lib()
     words = L.usdu_resample_table_words(in_size, out_size)

@@ -1,4 +1,4 @@
-// usdu_common.cuh -- shared declarations for libusdu_b200.so (sm_100a only).
+// usdu_common.cuh -- shared declarations for libusdu_b200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -16,6 +16,10 @@ constexpr int kThreads = 256;
 
 void set_error(const char* fmt, ...);
 int check_cuda(cudaError_t e, const char* what);
+// SMs of the current device (cudaDevAttrMultiProcessorCount, cached per device), or a negative usdu_status.
+int sm_count();
+// the same for sizing grids: at least 1 (a failed query leaves the error to the launch that follows)
+inline int grid_sms() { const int n = sm_count(); return n > 0 ? n : 1; }
 
 #define USDU_REQUIRE(cond, ...)                      \
     do {                                             \

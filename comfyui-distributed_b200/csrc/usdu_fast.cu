@@ -1,4 +1,4 @@
-// usdu_fast.cu -- fast crop+LANCZOS and LANCZOS-back+composite kernels (sm_100a).
+// usdu_fast.cu -- fast crop+LANCZOS and LANCZOS-back+composite kernels (sm_90a).
 // See usdu_fast.cuh for the engine; this file holds staging, epilogues and launchers.
 #include "usdu_fast.cuh"
 #include "usdu_tma.cuh"

@@ -1,14 +1,14 @@
 // usdu_fast.cuh -- the two-pass 8-bit LANCZOS engine shared by the fast crop and blend
-// kernels (sm_100a).
+// kernels (sm_90a).
 //
-// Cost model (measured on B200, tools/ubench/pipes.cu): IMAD issues at 64 lanes/clk/SM, byte
+// Cost model (tools/ubench/pipes.cu measures it): IMAD issues at 64 lanes/clk/SM, byte
 // extraction (PRMT) at 64, and every instruction takes one of the 128 issue slots/clk/SM.
 // The naive form -- one shared-memory byte load + one IMAD per tap -- needs ~300 thread
 // instructions per output byte.  Here one 32-bit shared-memory load brings the tap's byte
 // of FOUR independent lines (rows in the H pass, byte columns in the V pass), so a tap costs
 // 1/4 LDS + PRMT + IMAD per byte, registers stay <= 64 and no dynamic register indexing is
-// needed.  (A register-window variant with a warp-uniform switch was measured first: 63
-// instr/byte at 16 warps/SM -- profiles/r01c_*; this form is simpler and faster.)
+// needed.  (A register-window variant with a warp-uniform switch needs more instructions per
+// byte and dynamic register indexing; this form is simpler.)
 //
 //   H pass  thread = output pixel column (coefficients in registers), loop over (group of 4
 //           rows, channel).  Input is staged PLANAR and ROW-PACKED: word(g, c, x) = bytes of
@@ -71,7 +71,7 @@ __device__ __forceinline__ void dot4(const uint32_t (&w)[N], const PackedRow<TAP
 #pragma unroll
     for (int t = 0; t < N; ++t) {
         // (moving one of the four extractions to the integer-FMA pipe with IMAD.HI -- hi32(w*2^8)
-        // == w >> 24 -- was measured and is slower: crop +4 %, blend +6 %)
+        // == w >> 24 -- would put more work on the already busier IMAD pipe)
 #pragma unroll
         for (int r = 0; r < R; ++r) acc[r] += (int)__byte_perm(w[t], 0, 0x4440 + r) * row.k[t];
     }

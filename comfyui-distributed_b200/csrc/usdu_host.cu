@@ -10,6 +10,7 @@
 #include <stdarg.h>
 #include <string.h>
 
+#include <atomic>
 #include <vector>
 
 #include "usdu_common.cuh"
@@ -31,6 +32,26 @@ int check_cuda(cudaError_t e, const char* what) {
     return USDU_ERR_CUDA;
 }
 
+int sm_count() {
+    static std::atomic<int> cache[64];
+    int dev = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    const bool cached = e == cudaSuccess && dev >= 0 && dev < 64;
+    if (cached) {
+        const int c = cache[dev].load(std::memory_order_relaxed);
+        if (c > 0) return c;
+    }
+    int n = 0;
+    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+    if (e != cudaSuccess) {
+        check_cuda(e, "cudaDeviceGetAttribute(cudaDevAttrMultiProcessorCount)");
+        cudaGetLastError();
+        return USDU_ERR_CUDA;
+    }
+    if (cached) cache[dev].store(n, std::memory_order_relaxed);
+    return n;
+}
+
 }  // namespace usdu
 
 extern "C" {
@@ -38,6 +59,8 @@ extern "C" {
 int usdu_abi_version(void) { return USDU_ABI_VERSION; }
 
 const char* usdu_last_error(void) { return usdu::g_err; }
+
+int usdu_sm_count(void) { return usdu::sm_count(); }
 
 int usdu_device_count(void) {
     int n = 0;

@@ -1,4 +1,4 @@
-// usdu_kernels.cu -- sm_100a kernels of the USDU tile path and their C-ABI launchers.
+// usdu_kernels.cu -- sm_90a kernels of the USDU tile path and their C-ABI launchers.
 //
 // All pixel arithmetic is integer and bit-exact with the reference's Pillow path
 // (specs V1-V5 in SURVEY.md section 8a, restated in oracle/usdu_oracle.py):
@@ -486,7 +486,7 @@ mask_expand_kernel(const MaskSpecDev* __restrict__ specs, const uint8_t* __restr
 }
 
 static inline int grid_for(int64_t blocks) {
-    const int64_t cap = 148 * 16;
+    const int64_t cap = (int64_t)grid_sms() * 16;
     return (int)(blocks < 1 ? 1 : (blocks > cap ? cap : blocks));
 }
 
@@ -535,10 +535,11 @@ int usdu_quantize_rows(const float* img_dev, uint8_t* canvas_dev, int B, int H, 
     const int W3 = W * 3;
     const int vec_ok = (W3 % 4 == 0) && (((uintptr_t)img_dev & 15) == 0) && (((uintptr_t)canvas_dev & 15) == 0);
     const int64_t total = (int64_t)B * (y1 - y0) * ((W3 + 15) / 16);
-    // short-lived CTAs (up to 148 x 128 of them, ~1 trip each on the 8K canvas): when this pass runs on a side stream beside
+    // short-lived CTAs (up to 128 per SM, ~1 trip each on the 8K canvas): when this pass runs on a side stream beside
     // small tile waves (engine.OverlappedJob) SM slots turn over every microsecond instead of being held for the whole pass
     const int64_t qblocks = (total + kThreads - 1) / kThreads;
-    const int grid = (int)(qblocks < 1 ? 1 : (qblocks > 148 * 128 ? 148 * 128 : qblocks));
+    const int64_t qcap = (int64_t)grid_sms() * 128;
+    const int grid = (int)(qblocks < 1 ? 1 : (qblocks > qcap ? qcap : qblocks));
     quantize_canvas_kernel<<<grid, kThreads, 0, (cudaStream_t)stream>>>(img_dev, canvas_dev, B * (y1 - y0), W3, pitch, vec_ok, H, y0, y1 - y0);
     USDU_CUDA(cudaGetLastError());
     return USDU_OK;
@@ -564,7 +565,8 @@ int usdu_dequantize_rows(const uint8_t* canvas_dev, float* img_dev, int B, int H
     if (gx < 1) gx = 1;
     int64_t gy = (int64_t)B * (y1 - y0);
     if (gy > 65535) gy = 65535;
-    if (gy * gx > 148 * 128) gy = (148 * 128 + gx - 1) / gx;       // short-lived CTAs, see usdu_quantize_rows
+    const int64_t qcap = (int64_t)grid_sms() * 128;                 // short-lived CTAs, see usdu_quantize_rows
+    if (gy * gx > qcap) gy = (qcap + gx - 1) / gx;
     if (gy < 1) gy = 1;
     dequantize_canvas_kernel<<<dim3(gx, (unsigned)gy), kThreads, 0, (cudaStream_t)stream>>>(canvas_dev, img_dev, B * (y1 - y0), W3, pitch, vec_ok, H, y0, y1 - y0);
     USDU_CUDA(cudaGetLastError());

@@ -1,12 +1,14 @@
-// usdu_mma.cu -- tensor-core crop+LANCZOS and LANCZOS-back+composite kernels (sm_100a).
+// usdu_mma.cu -- tensor-core crop+LANCZOS and LANCZOS-back+composite kernels (sm_90a).
 //
 // Pillow's 8-bit resampling pass is a banded integer contraction, out[o] = clip8((2^21 + sum_k in[k] * coef[o][k]) >> 22)
 // with 23-bit signed coefficients.  On the CUDA-core integer pipes a tap costs one PRMT + one IMAD per byte
-// (usdu_fast.cuh: 5.0 output bytes/clk/SM, the kernels were ALU-pipe bound at 0.20 of the HBM roofline).  Here the taps
+// (usdu_fast.cuh), so the CUDA-core kernels are ALU-pipe bound, far from the HBM roofline.  Here the taps
 // run on the tensor cores: mma.sync.m16n8k32 multiplies u8 pixels by 8-bit LIMBS of the coefficients
 // (coef = l2 * 65536 + l1 * 256 + l0; l0, l1 unsigned, l2 signed) with exact s32 accumulation, three IMMAs per
 // 16 x 8 x 32 tile, recombined with two shift-adds.  |limb sum| <= 64 * 255 * 255 < 2^23, and the recombined value is
-// Pillow's accumulator exactly, so the results stay bit-identical (tools/ubench/imma.cu: probe + 7.7 / 9.5 B/clk/SM).
+// Pillow's accumulator exactly, so the results stay bit-identical (tools/ubench/imma.cu: probe + throughput).
+// Hopper's integer wgmma (s8/u8, m64nNk32) would need the pixel operand in shared memory in its core-matrix layout and a
+// warpgroup per 64 output rows; the patches here are 16-row M-tiles of 1 or 2 k-steps, so the warp-level IMMA stays.
 //
 // Both passes put the COEFFICIENTS in the A operand (16 outputs x 32 inputs, built on the host in fragment order:
 // planner.build_mma_frags) and the PIXELS in B:
@@ -26,12 +28,11 @@ namespace usdu {
 namespace mma {
 
 constexpr int kT = 256;                     // 8 warps
-// Resident CTAs per SM the kernels are compiled for.  3 = 80 registers, no spills: the faster build inside the 31-wave job,
-// where launches are 1-8 tiles and per-thread speed counts (cfg2: 1.222 vs 1.270 ms).  4 = 64 registers: more warps to hide the
-// staging latency, the faster build for the CROP on machine-filling launches (all 135 tiles: 216 vs 234 us); the blend gains
-// nothing from it (331 vs 333 us).  The crop launcher picks by grid size; profiles/r02n_*, r02o_*.
+// Resident CTAs per SM the kernels are compiled for.  3 = 80 registers: more registers per thread for the small launches
+// of the wave loop (1-8 tiles), where per-thread speed counts.  4 = 64 registers: more warps to hide the staging latency on
+// machine-filling crop launches.  The crop launcher picks by grid size.
 constexpr int kOccSmall = 3, kOccLarge = 4;
-constexpr int kLargeGrid = 148 * 8;          // CTAs from which the 4-CTA build of the crop is used
+constexpr int kLargeGridPerSM = 8;          // CTAs per SM from which the 4-CTA build of the crop is used
 constexpr int BWX = USDU_FAST_BLOCK_W;      // 128-pixel wide blocks
 constexpr int MIDP = 440;                   // words per row group of the intermediate: >= 3 * 144 columns, == 24 mod 32
 constexpr int kDBox = BWX * 3 / 2;          // canvas block = two bulk-tensor boxes of 192 bytes per row
@@ -789,7 +790,7 @@ int launch_crop(const void* canvas, int src_f32, int B, int H, int W, int64_t pi
     const uint8_t* cv = static_cast<const uint8_t*>(canvas);
     const dim3 grid(n_items, B);
     const int W3 = W * 3;
-    const bool large = (int64_t)n_items * B >= kLargeGrid && !two_ksteps;
+    const bool large = (int64_t)n_items * B >= (int64_t)kLargeGridPerSM * grid_sms() && !two_ksteps;
 #define USDU_CROP_LAUNCH(SRC)                                                                                                                   \
     (two_ksteps ? launch_one(crop_mma_kernel<SRC, 2, kOccSmall>, smem, grid, st, cv, H, pitch, tabs, items, out, patch_w, plane_rows, mid_rows, W3, cmap) \
      : large    ? launch_one(crop_mma_kernel<SRC, 1, kOccLarge>, smem, grid, st, cv, H, pitch, tabs, items, out, patch_w, plane_rows, mid_rows, W3, cmap) \

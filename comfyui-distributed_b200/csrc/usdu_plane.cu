@@ -148,7 +148,7 @@ pad_fill_kernel(PlaneView src, int n, int h, int w, int hp, int vp, const int32_
 
 static inline int grid_of(int64_t work_items) {
     int64_t blocks = (work_items + kThreads - 1) / kThreads;
-    const int64_t cap = 148 * 8;
+    const int64_t cap = (int64_t)grid_sms() * 8;
     if (blocks > cap) blocks = cap;
     if (blocks < 1) blocks = 1;
     return (int)blocks;

@@ -1,4 +1,4 @@
-// usdu_tma.cuh -- Tensor Memory Accelerator plumbing (sm_100a): 2-D tiled tensor maps over the
+// usdu_tma.cuh -- Tensor Memory Accelerator plumbing (sm_90a): 2-D tiled tensor maps over the
 // u8 canvas, bulk-tensor loads into shared memory signalled through an mbarrier, bulk-tensor
 // stores back.  Inline PTX only (no CUTLASS); the host encoder is resolved through
 // cudaGetDriverEntryPoint so the library does not link libcuda.

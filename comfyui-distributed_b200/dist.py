@@ -1,4 +1,4 @@
-"""Multi-GPU plumbing: one process per GPU, torch.distributed (NCCL over NVLink 5 /
+"""Multi-GPU plumbing: one process per GPU, torch.distributed (NCCL over NVLink 4 /
 NVSwitch; gloo in the CPU tests).  Replaces the reference's HTTP + PNG transport:
 
 * upscale/worker_comms.py:16-108  (PNG multipart POST of processed tiles)  and
@@ -209,8 +209,8 @@ class StaticJob:
         # with a conflict-free partition no crop of this rank ever sees one of its own blends and, when the final
         # canvas is composited slab by slab from the payloads, nobody reads this rank's working canvas: skip them
         self.skip = ("blend",) if (self.sharded and self.conflict_free) else ()
-        # ... and then its crops can read the fp32 image directly: the whole-canvas quantise (90 us of every rank's step on
-        # the 8K canvas, never sharded) disappears from the device-resident path
+        # ... and then its crops can read the fp32 image directly: the whole-canvas quantise (a pass over the whole canvas
+        # in every rank's step, never sharded) disappears from the device-resident path
         self.from_image = bool(self.skip) and Canvas(self.dp, B, self.work_buf).can_crop_image() and len(self.asg[self.rank]) > 0
         self.gw = None
         if self.graphed:
@@ -477,7 +477,7 @@ class SharedHost:
         return sum(1 for lst in self.bufs.values() for i in range(len(lst)) if lst[i] is not None)
 
     def _map(self, numel: int, k: int, touch: Optional[Tuple[int, int]] = None) -> torch.Tensor:
-        """Buffer k of `numel` floats: mapped and page-locked on first use (~150 ms for 400 MB, once), COLLECTIVELY (every
+        """Buffer k of `numel` floats: mapped and page-locked on first use (once: page locking is slow), COLLECTIVELY (every
         rank maps a new buffer in the same job, see begin()).  touch = (a, b): element range this rank will write -- it
         is first-touched here."""
         lst = self.bufs.setdefault(numel, [])
@@ -489,8 +489,7 @@ class SharedHost:
             if touch is not None:
                 # First touch decides which NUMA node a page of the shared buffer lives on.  Every rank touches the rows IT
                 # will download into, on a CPU next to its GPU: otherwise all pages sit next to rank 0 and the GPUs of the
-                # other socket write across the inter-socket link (measured on this 2-socket box: 4.2 ms instead of ~1 ms
-                # for a 50 MB slab with 4 of 8 GPUs on the far socket).
+                # other socket write across the inter-socket link, several times slower than writes to local memory.
                 a, b = touch
                 with _near_gpu_cpus():
                     t.view(-1)[a:b].zero_()

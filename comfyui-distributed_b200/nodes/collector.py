@@ -124,7 +124,7 @@ class DistributedCollectorNode:
                 # started as an HTTP worker of the reference's orchestrator: there is no torch.distributed peer to send the
                 # batch to, and the reference's HTTP collection is not part of this package -- say so instead of dropping it
                 import warnings
-                warnings.warn("DistributedCollector (B200): running as an HTTP worker of the reference's orchestrator is not "
+                warnings.warn("DistributedCollector (CUDA tile path): running as an HTTP worker of the reference's orchestrator is not "
                               "supported (launch one rank per GPU with torch.distributed); this worker's images stay local.",
                               RuntimeWarning, stacklevel=2)
             return (images, audio if audio is not None else empty_audio)

@@ -1,9 +1,9 @@
 """UltimateSDUpscaleDistributed -- same ComfyUI node signature as the reference's
-nodes/distributed_upscale.py:46-279, running the tile path on the B200 kernels.
+nodes/distributed_upscale.py:46-279, running the tile path on the H100 kernels.
 
 What changes behind the signature:
 * pixels never touch PIL or the CPU: the canvas lives in HBM as u8, crop / feather /
-  blend are sm_100a kernels (engine.py);
+  blend are sm_90a kernels (engine.py);
 * "workers" are torch.distributed ranks (one process per GPU, NCCL); the hidden inputs
   injected by the reference's orchestrator (multi_job_id, is_worker, master_url,
   enabled_worker_ids, worker_id, tile_indices, dynamic_threshold) are accepted and
@@ -118,7 +118,7 @@ class UltimateSDUpscaleDistributed:
             # and PNG transport are not part of this package (an SPMD launch, one rank per GPU, replaces them): do what
             # a worker does for the graph -- hand the input through (static.py:314) -- and say why no tile was processed.
             import warnings
-            warnings.warn("UltimateSDUpscaleDistributed (B200): running as an HTTP worker of the reference's orchestrator is "
+            warnings.warn("UltimateSDUpscaleDistributed (CUDA tile path): running as an HTTP worker of the reference's orchestrator is "
                           "not supported; launch one rank per GPU with torch.distributed instead. Returning the input.",
                           RuntimeWarning, stacklevel=2)
             return (upscaled_image,)

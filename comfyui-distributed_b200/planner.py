@@ -500,7 +500,13 @@ class Plan:
         ends = np.minimum(starts + block, n_out) - 1
         return int((sp[ends, 1] - sp[starts, 0]).max())
 
-    SLOTS = 148 * 4            # resident CTAs of the fast kernels on a B200 (4 per SM)
+    CTAS_PER_SM = 4            # resident CTAs of the fast kernels per SM
+    DEFAULT_SMS = 132          # H100 SXM: the block shapes of plans made where no device can be queried
+
+    @classmethod
+    def resident_slots(cls) -> int:
+        """Resident CTAs of the fast kernels on the current device (nat.sm_count(), the SM count the launchers see)."""
+        return (nat.sm_count() or cls.DEFAULT_SMS) * cls.CTAS_PER_SM
 
     def block_shape(self, use_fast: bool, extents: Optional[Sequence[Tuple[int, int]]] = None, frames: int = 1,
                     share: int = 1, mma: bool = False) -> Tuple[int, int]:
@@ -516,10 +522,11 @@ class Plan:
         if not extents:
             return bw, nat.FAST_BLOCK_H
         best = None
+        slots = self.resident_slots()
         forced = os.environ.get("USDU_MMA_BH") if mma else None            # experiments: force the tensor-core block height
         for bh in (((int(forced),) if forced else (16, 32)) if mma else (8, 12, 16, 20, 24, 28, 32)):   # M-tiles are 16 output rows
             n = sum(((w + bw - 1) // bw + 1) * ((h + bh - 1) // bh + 1) for w, h in extents) * frames   # +1: unaligned windows
-            cost = math.ceil(n / max(self.SLOTS // max(share, 1), 1)) * (bh + 12)
+            cost = math.ceil(n / max(slots // max(share, 1), 1)) * (bh + 12)
             if best is None or cost < best[0] or (cost == best[0] and bh > best[1]):
                 best = (cost, bh)
         return bw, best[1]

@@ -1,5 +1,5 @@
 /*
- * usdu_b200.h -- C ABI of libusdu_b200.so: the B200-native (sm_100a) replacement for the
+ * usdu_b200.h -- C ABI of libusdu_b200.so: the H100-native (sm_90a) replacement for the
  * CPU/Pillow pixel path of ComfyUI-Distributed's Ultimate-SD-Upscale tile pipeline.
  *
  * The boundary is plain C: raw pointers, sizes, a CUDA stream handle passed as void*.
@@ -156,6 +156,8 @@ int usdu_abi_version(void);
 const char* usdu_last_error(void);
 /* number of CUDA devices visible, or a negative usdu_status */
 int usdu_device_count(void);
+/* streaming multiprocessors of the current CUDA device, or a negative usdu_status */
+int usdu_sm_count(void);
 
 /* ---- host-side table builders (exact Pillow arithmetic, C double / C float) -------- */
 /* taps per output for an in->out LANCZOS axis (Resample.c: ceil(3*max(in/out,1))*2+1) */

@@ -1,6 +1,7 @@
 """oracle.collector_combine == the reference's own DistributedCollector arithmetic (worker PNG round trip,
 master decode, _reorder_and_combine_tensors), loaded from /root/reference by oracle/ref_collector.py.
-Skipped where the reference tree is absent; tests/golden/collector_ref.json pins the same there."""
+Where the reference tree is absent, tests/golden/collector_ref.json and tests/golden/reference_results.json
+(tests/recorded.py) pin the same."""
 import hashlib
 import json
 import os
@@ -11,6 +12,7 @@ import torch
 
 import ref_collector
 import usdu_oracle as orc
+from recorded import digest, reference_digest
 
 G = os.path.join(os.path.dirname(__file__), "golden")
 CASES = json.load(open(os.path.join(G, "collector_ref.json")))["cases"]
@@ -42,17 +44,15 @@ def test_reference_collector_matches_golden_and_oracle(case):
     assert np.array_equal(out, ref)
 
 
-@pytest.mark.skipif(not ref_collector.available(), reason="reference tree not present")
 def test_audio_combination_matches_reference():
     """nodes/collector.py:121-174 side by side with our combine_audio on random piece sets (missing audio,
     empty waveforms, non-default sample rates, unexpected worker ids)."""
     from __graft_entry__ import load_package
     load_package()
     from comfyui_distributed_b200.nodes.collector import combine_audio
-    collector, _, _ = ref_collector.load()
-    node = collector.DistributedCollectorNode()
     empty = {"waveform": torch.zeros(1, 2, 1), "sample_rate": 44100}
     rng = np.random.default_rng(0)
+    cases = []
     for _ in range(200):
         def piece():
             k = rng.integers(0, 4)
@@ -64,8 +64,16 @@ def test_audio_combination_matches_reference():
         ids = ["w1", "w2", "w3", "zz"]
         workers = {w: piece() for w in ids if rng.random() < 0.8}
         order = [w for w in ["w2", "w1", "w3"] if rng.random() < 0.8]
-        ref = node._combine_audio(master, workers, empty, order)
+        cases.append((master, workers, order))
+
+    def reference():
+        collector, _, _ = ref_collector.load()
+        node = collector.DistributedCollectorNode()
+        return [(ref["sample_rate"], ref["waveform"]) for ref in (node._combine_audio(m, w, empty, o) for m, w, o in cases)]
+
+    got = []
+    for master, workers, order in cases:
         seq = [master] + [workers.get(w) for w in order] + [workers[w] for w in sorted(workers) if w not in order]
-        got = combine_audio(seq, empty)
-        assert got["sample_rate"] == ref["sample_rate"]
-        assert torch.equal(got["waveform"], ref["waveform"])
+        a = combine_audio(seq, empty)
+        got.append((a["sample_rate"], a["waveform"]))
+    assert digest(got) == reference_digest("collector/combine_audio/200_random_piece_sets", ref_collector.available(), reference)

@@ -73,7 +73,7 @@ def test_node_api_on_a_host_tensor_matches_the_reference_digest(name):
 
 def test_fused_level_launches_give_the_same_canvas():
     """engine.FUSE_LEVELS: blend(k) U crop(k+1) as one launch ordered by device-side ready counters
-    (usdu_level_blend_crop) -- off by default (measured slower), kept correct: same digest as the reference on cfg2."""
+    (usdu_level_blend_crop) -- off by default (not faster than the level loop), kept correct: same digest as the reference on cfg2."""
     B, H, W, tile, pad, blur = WORKLOADS["cfg2_4k_to_8k_sdxl_512px"]
     want = _expected("cfg2_4k_to_8k_sdxl_512px")
     img = _canvas(B, H, W).cuda()

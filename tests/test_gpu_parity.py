@@ -1,4 +1,4 @@
-"""GPU parity tests: the sm_100a kernels (through the C ABI / ctypes) against the oracle
+"""GPU parity tests: the sm_90a kernels (through the C ABI / ctypes) against the oracle
 and the committed golden fixtures.  Bit-exact (integer / byte work)."""
 import json
 import os

@@ -18,7 +18,7 @@ W = {"cfg2": (1, 4320, 7680, 512, 32, 8), "cfg4": (1, 8640, 15360, 256, 32, 8), 
 name = sys.argv[1] if len(sys.argv) > 1 else "cfg2"
 B, H, Wd, tile, pad, blur = W[name]
 peak = json.load(open(os.path.join(os.path.dirname(__file__), "..", "MEASURED_PEAKS.json")))["hbm_gbs"] if os.path.isfile(
-    os.path.join(os.path.dirname(__file__), "..", "MEASURED_PEAKS.json")) else 6650.0
+    os.path.join(os.path.dirname(__file__), "..", "MEASURED_PEAKS.json")) else 3350.0   # H100 SXM data sheet
 plan = planner.get_plan(Wd, H, tile, tile, pad, blur, True)
 dev = torch.device("cuda", 0)
 img = torch.rand(B, H, Wd, 3, device=dev)

@@ -1,4 +1,4 @@
-"""Static SASS opcode histogram per kernel of libusdu_b200.so (what proves a Blackwell-native kernel: UTMALDG / UTMASTG =
+"""Static SASS opcode histogram per kernel of libusdu_b200.so (what proves a Hopper-native kernel: UTMALDG / UTMASTG =
 TMA bulk-tensor loads / stores, IMMA = mma.sync int8 tensor cores, I2IP = cvt.pack.sat, SYNCS / mbarrier traffic,
 griddepcontrol = programmatic dependent launch).   python tools/sass_hist.py [out.json]"""
 import collections

@@ -1,4 +1,4 @@
-// Tensor-core formulation of one 8-bit LANCZOS pass (B200, sm_100a): probe + shoot-out.
+// Tensor-core formulation of one 8-bit LANCZOS pass (H100, sm_90a): probe + shoot-out.
 //
 // A resampling pass is a banded integer contraction: out[o] = (2^21 + sum_k in[k] * coef[o][k]) >> 22 with 23-bit
 // signed coefficients.  mma.sync.m16n8k32 multiplies u8 pixels by 8-bit coefficient LIMBS with exact s32
@@ -9,9 +9,9 @@
 //   part 2  raw IMMA issue rate (independent accumulators)
 //   part 3  H pass:  M = 16 outputs (coefficient band matrix, registers), N = rows, K = 32 input pixels of a plane
 //           V pass:  M = 16 output rows (coefficients, registers), N = byte columns, K = 32 input rows (row-packed)
-//           reported as output bytes/clk/SM, to compare with taps.cu's "A prmt+imad" (5.02 on B200)
+//           reported as output bytes/clk/SM, to compare with taps.cu's "A prmt+imad"
 //
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o imma imma.cu && ./imma
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o imma imma.cu && ./imma
 #include <cstdio>
 #include <cstdlib>
 #include <cuda_runtime.h>
@@ -212,30 +212,30 @@ int main() {
             }
         printf("probe: %d of 128 outputs differ from the scalar loop (%s)\n", bad, cudaGetErrorString(cudaGetLastError()));
     }
-    cudaMalloc(&g_out, 148 * 4 * 256 * 4);
+    cudaMalloc(&g_out, 132 * 4 * 256 * 4);
     cudaMalloc(&g_frags, 64 * 32 * 16); cudaMemset(g_frags, 0x11, 64 * 32 * 16);
     cudaMalloc(&g_kx0, 64); cudaMemset(g_kx0, 0, 64);
-    const double clk = 1.965e9;
+    const double clk = 1.98e9;
     // ---- part 2 ----
     {
-        float ms = timeit([] { rate<<<148 * 4, 256>>>(g_out, 8); });
-        const double n = 148.0 * 4 * 8 * ITERS * 16 * 8;     // warp-level MMAs
-        printf("IMMA.16832 u8: %.3f ms  %.3f MMA/clk/SM  = %.0f MAC/clk/SM  (%.1f TOPS dense at 1.965 GHz)\n", ms,
-               n / (ms * 1e-3 * clk) / 148, n / (ms * 1e-3 * clk) / 148 * 4096, n * 4096 * 2 / (ms * 1e-3) / 1e12);
+        float ms = timeit([] { rate<<<132 * 4, 256>>>(g_out, 8); });
+        const double n = 132.0 * 4 * 8 * ITERS * 16 * 8;     // warp-level MMAs
+        printf("IMMA.16832 u8: %.3f ms  %.3f MMA/clk/SM  = %.0f MAC/clk/SM  (%.1f TOPS dense at 1.98 GHz)\n", ms,
+               n / (ms * 1e-3 * clk) / 132, n / (ms * 1e-3 * clk) / 132 * 4096, n * 4096 * 2 / (ms * 1e-3) / 1e12);
     }
     // ---- part 3 ----
     {
         const int smH = 3 * 40 * PB + 160 + 12 * MIDP * 4;
         cudaFuncSetAttribute(kH, cudaFuncAttributeMaxDynamicSharedMemorySize, smH);
         static int s_smH; s_smH = smH;
-        float ms = timeit([] { kH<<<148 * 4, 256, s_smH>>>(g_out, g_frags, g_kx0); });
+        float ms = timeit([] { kH<<<132 * 4, 256, s_smH>>>(g_out, g_frags, g_kx0); });
         // per CTA per iter: 3 channels x 40 rows x 128 px outputs (48 rows computed, 40 valid)
         printf("H pass (IMMA): %.3f ms  %.2f output bytes/clk/SM (valid rows)  [smem %d B]  (%s)\n", ms,
                3.0 * 40 * 128 * ITERS * 4 / (ms * 1e-3 * clk), smH, cudaGetErrorString(cudaGetLastError()));
         const int smV = 10 * MIDP * 4 + 32 * 384;
         cudaFuncSetAttribute(kV, cudaFuncAttributeMaxDynamicSharedMemorySize, smV);
         static int s_smV; s_smV = smV;
-        ms = timeit([] { kV<<<148 * 4, 256, s_smV>>>(g_out, g_frags); });
+        ms = timeit([] { kV<<<132 * 4, 256, s_smV>>>(g_out, g_frags); });
         printf("V pass (IMMA): %.3f ms  %.2f output bytes/clk/SM  [smem %d B]  (%s)\n", ms,
                32.0 * 384 * ITERS * 4 / (ms * 1e-3 * clk), smV, cudaGetErrorString(cudaGetLastError()));
     }

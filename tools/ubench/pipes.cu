@@ -1,5 +1,5 @@
-// Pipe-throughput microbenchmark (B200): which integer/fp MAC form is fastest per SM?
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o pipes pipes.cu && ./pipes
+// Pipe-throughput microbenchmark (H100): which integer/fp MAC form is fastest per SM?
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o pipes pipes.cu && ./pipes
 #include <cstdio>
 #include <cuda_runtime.h>
 #define ITERS 4096
@@ -30,15 +30,15 @@ __global__ void k(int* out, int a0, int b0, float fa, float fb) {
     out[blockIdx.x * blockDim.x + threadIdx.x] = s + (int)fs;
 }
 template <int MODE> void run(const char* name, int ops_per_iter) {
-    int* out; cudaMalloc(&out, 148 * 8 * 1024 * sizeof(int));
+    int* out; cudaMalloc(&out, 132 * 8 * 1024 * sizeof(int));
     cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
-    k<MODE><<<148 * 8, 256>>>(out, 1, 2, 1.f, 2.f);
+    k<MODE><<<132 * 8, 256>>>(out, 1, 2, 1.f, 2.f);
     cudaEventRecord(e0);
-    k<MODE><<<148 * 8, 256>>>(out, 1, 2, 1.f, 2.f);
+    k<MODE><<<132 * 8, 256>>>(out, 1, 2, 1.f, 2.f);
     cudaEventRecord(e1); cudaEventSynchronize(e1);
     float ms; cudaEventElapsedTime(&ms, e0, e1);
-    double n = 148.0 * 8 * 256 * ITERS * 8 * ops_per_iter;
-    printf("%-28s %8.3f ms  %8.2f Tlane-op/s  (%.1f lane-ops/clk/SM @1.965GHz)\n", name, ms, n / ms / 1e9, n / (ms * 1e-3) / 148 / 1.965e9);
+    double n = 132.0 * 8 * 256 * ITERS * 8 * ops_per_iter;
+    printf("%-28s %8.3f ms  %8.2f Tlane-op/s  (%.1f lane-ops/clk/SM @1.98GHz)\n", name, ms, n / ms / 1e9, n / (ms * 1e-3) / 132 / 1.98e9);
     cudaFree(out);
 }
 int main() {

@@ -1,4 +1,4 @@
-// Which pipe does IDP.4A share?  nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o pipes2 pipes2.cu
+// Which pipe does IDP.4A share?  nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o pipes2 pipes2.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 #define ITERS 4096
@@ -24,15 +24,15 @@ __global__ void k(int* out, int a0, int b0) {
     out[blockIdx.x * blockDim.x + threadIdx.x] = s;
 }
 template <int MODE> void run(const char* name, int ops) {
-    int* out; cudaMalloc(&out, 148 * 8 * 256 * sizeof(int));
+    int* out; cudaMalloc(&out, 132 * 8 * 256 * sizeof(int));
     cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
-    k<MODE><<<148 * 8, 256>>>(out, 1, 2);
+    k<MODE><<<132 * 8, 256>>>(out, 1, 2);
     cudaEventRecord(e0);
-    k<MODE><<<148 * 8, 256>>>(out, 1, 2);
+    k<MODE><<<132 * 8, 256>>>(out, 1, 2);
     cudaEventRecord(e1); cudaEventSynchronize(e1);
     float ms; cudaEventElapsedTime(&ms, e0, e1);
-    double n = 148.0 * 8 * 256 * ITERS * 8 * ops;
-    printf("%-28s %8.3f ms  %.1f lane-ops/clk/SM\n", name, ms, n / (ms * 1e-3) / 148 / 1.965e9);
+    double n = 132.0 * 8 * 256 * ITERS * 8 * ops;
+    printf("%-28s %8.3f ms  %.1f lane-ops/clk/SM\n", name, ms, n / (ms * 1e-3) / 132 / 1.98e9);
     cudaFree(out);
 }
 int main() {

@@ -1,4 +1,4 @@
-// Inner-loop shoot-out for one resampling pass over shared memory (B200):
+// Inner-loop shoot-out for one resampling pass over shared memory (H100):
 //   A: current scheme  -- LDS.32 = 1 tap of 4 lines, PRMT + IMAD per tap and line (7 taps)
 //   B: dp4a scheme     -- per output byte: 3 LDS.32, 2 funnel shifts, 6 IDP.4A (8 taps, 3 coefficient planes)
 // Both produce u8 outputs into shared memory; bytes/clk/SM reported.  256 thr x 4 CTAs/SM.
@@ -73,12 +73,12 @@ __global__ void __launch_bounds__(256, 4) kB(int* out, const int* coef) {
 }
 
 template <class F> void run(const char* name, F f, double bytes_per_iter) {
-    int *out, *coef; cudaMalloc(&out, 148 * 4 * 256 * 4); cudaMalloc(&coef, 128 * 8 * 4); cudaMemset(coef, 1, 128 * 8 * 4);
+    int *out, *coef; cudaMalloc(&out, 132 * 4 * 256 * 4); cudaMalloc(&coef, 128 * 8 * 4); cudaMemset(coef, 1, 128 * 8 * 4);
     cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
-    f<<<148 * 4, 256>>>(out, coef);
-    cudaEventRecord(e0); f<<<148 * 4, 256>>>(out, coef); cudaEventRecord(e1); cudaEventSynchronize(e1);
+    f<<<132 * 4, 256>>>(out, coef);
+    cudaEventRecord(e0); f<<<132 * 4, 256>>>(out, coef); cudaEventRecord(e1); cudaEventSynchronize(e1);
     float ms; cudaEventElapsedTime(&ms, e0, e1);
-    printf("%-10s %8.3f ms  %.2f output bytes/clk/SM  (%s)\n", name, ms, bytes_per_iter * ITERS * 4 / (ms * 1e-3 * 1.965e9), cudaGetErrorString(cudaGetLastError()));
+    printf("%-10s %8.3f ms  %.2f output bytes/clk/SM  (%s)\n", name, ms, bytes_per_iter * ITERS * 4 / (ms * 1e-3 * 1.98e9), cudaGetErrorString(cudaGetLastError()));
 }
 int main() {
     run("A prmt+imad", kA, 30.0 * 4 * 128);     // per CTA per iter: 30 units x 4 rows x 128 px bytes
