@@ -57,7 +57,8 @@ __device__ __forceinline__ void stage_u8(uint32_t* __restrict__ in, int xw, cons
 }
 
 // fp32 source in [0,1] -> quantise (Q1) -> planar row-packed.  src points at the first float of
-// a 12-float (4 pixel) aligned chunk that contains the patch start; lead = pixels before it.
+// a 12-float (4 pixel) aligned chunk that contains the patch start; lead = pixels before it.  Evict-first loads: the
+// source is dead once blended (see usdu_mma.cu stage_f32).
 __device__ __forceinline__ void stage_f32(uint32_t* __restrict__ in, int xw, const float* __restrict__ src,
                                           int64_t pitch_f, int rows, int rows_valid, int px_count, int lead) {
     const int chunks = (px_count + lead + 3) >> 2;
@@ -71,7 +72,7 @@ __device__ __forceinline__ void stage_f32(uint32_t* __restrict__ in, int xw, con
             const float4* p = reinterpret_cast<const float4*>(src + (int64_t)rr * pitch_f) + ch * 3;
 #pragma unroll
             for (int k = 0; k < 3; ++k) {
-                const float4 f = __ldg(p + k);
+                const float4 f = __ldcs(p + k);
                 q[r][k] = quant_u8(f.x) | (quant_u8(f.y) << 8) | (quant_u8(f.z) << 16) | (quant_u8(f.w) << 24);
             }
         }
@@ -199,7 +200,7 @@ struct CropEpilogue {
         if (4 * strip < ow3) {   // ow3 is a multiple of 4 (pw % 8 == 0)
             float4 o;
             o.x = lut[s[0]]; o.y = lut[s[1]]; o.z = lut[s[2]]; o.w = lut[s[3]];
-            __stcs(reinterpret_cast<float4*>(dst + (int64_t)r * row_pitch + 4 * strip), o);
+            store_handoff(dst + (int64_t)r * row_pitch + 4 * strip, o);
         }
     }
 };

@@ -264,6 +264,8 @@ __device__ __forceinline__ int div_u16(int i, uint32_t m) { return m ? (int)__um
 
 // fp32 source in [0,1] (sampler output): Q1 truncation on the fly.  src -> first float of the staged patch.
 // kU units per thread per trip, every load issued before the first use (12 x 16 bytes in flight per thread).
+// Evict-first loads (__ldcs): the sampler output is dead once blended, so its lines should leave L2 before the next wave's
+// crop output, which the next sampler reads (DESIGN section 9.1).
 __device__ __forceinline__ void stage_f32(uint8_t* planes, int PB, int plane_rows, const float* __restrict__ src, int64_t pitch_f,
                                           int rows, int cols) {
     constexpr int kU = 4;                       // 1024 units per trip: a 128 x 16 block (<= 825 units) is staged in ONE round of loads
@@ -277,7 +279,7 @@ __device__ __forceinline__ void stage_f32(uint8_t* planes, int PB, int plane_row
             const int i = min(i0 + u * kT, total - 1);
             rr[u] = div_u16(i, rc); cc[u] = i - rr[u] * chunks;
             const float4* p = reinterpret_cast<const float4*>(src + (int64_t)rr[u] * pitch_f) + cc[u] * 3;
-            f[u][0] = __ldg(p); f[u][1] = __ldg(p + 1); f[u][2] = __ldg(p + 2);
+            f[u][0] = __ldcs(p); f[u][1] = __ldcs(p + 1); f[u][2] = __ldcs(p + 2);
         }
 #pragma unroll
         for (int u = 0; u < kU; ++u) {
@@ -368,7 +370,7 @@ struct CropEpilogue {
             float4 o;
             o.x = dequant_u8_fast(v & 0xFF); o.y = dequant_u8_fast((v >> 8) & 0xFF);
             o.z = dequant_u8_fast((v >> 16) & 0xFF); o.w = dequant_u8_fast(v >> 24);
-            __stcs(reinterpret_cast<float4*>(rp[h] + 4 * strip), o);
+            store_handoff(rp[h] + 4 * strip, o);
         }
     }
 };
