@@ -19,6 +19,8 @@ from typing import Optional, Sequence, Tuple
 import torch
 import torch.nn.functional as F
 
+from .casts import reference_f32
+
 Region = Tuple[int, int, int, int]
 
 
@@ -181,7 +183,7 @@ class MaskCropper:
         hit = self._masks.get(id(mask))
         if hit is not None and hit[0] is mask:
             return hit[1]
-        x = mask.detach().to(torch.float32)
+        x = reference_f32(mask.detach())
         if not x.is_cuda:
             x = x.contiguous()
             x = (x if x.is_pinned() else x.pin_memory()).to(self.device, non_blocking=True)

@@ -36,9 +36,15 @@ inline int grid_sms() { const int n = sm_count(); return n > 0 ? n : 1; }
     } while (0)
 
 // (uint8)(255.f * x): fp32 multiply (round to nearest), C truncation, wrap to 8 bits.
-// utils/image.py:8-10 -- numpy's float32 -> uint8 cast on x86 (cvttss2si, low byte).
+// utils/image.py:8-10 -- numpy's float32 -> uint8 cast on x86: cvttss2si, then the low byte.  cvttss2si returns
+// 0x80000000 for NaN, +-inf and every product outside [-2^31, 2^31), so all of those give 0.  cvt.rzi.s32 gives 0
+// for NaN and 0x80000000 below the range, but saturates to 0x7FFFFFFF above it (255 for the low byte), so products
+// >= 2^31 (and +inf) are replaced by 0 before the conversion: one FSETP + FSEL, and the bytes are still packed with
+// PRMT (a compare on the integer result costs more and made blend_fast_kernel spill).  Checked against numpy's rule
+// for all 2^32 fp32 inputs in tests/test_gpu_casts.py.
 __device__ __forceinline__ uint32_t quant_u8(float x) {
-    return static_cast<uint32_t>(__float2int_rz(__fmul_rn(255.0f, x))) & 0xFFu;
+    const float p = __fmul_rn(255.0f, x);
+    return static_cast<uint32_t>(__float2int_rz(p < 2147483648.0f ? p : 0.0f)) & 0xFFu;
 }
 
 // u / 255.0f with IEEE division (utils/image.py:13).

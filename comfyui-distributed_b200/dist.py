@@ -24,6 +24,7 @@ import numpy as np
 import torch
 import torch.distributed as td
 
+from .casts import reference_f32
 from .lru import LruCache
 
 
@@ -590,7 +591,7 @@ def upscale_static_host(host_image: torch.Tensor, denoiser, tile_width: int, til
 
     rank, world = dist_info(group)
     device = device or torch.device("cuda", torch.cuda.current_device())
-    x = host_image.to(torch.float32).contiguous()
+    x = reference_f32(host_image).contiguous()
     B, H, W, _ = x.shape
     plan = get_plan(W, H, tile_width, tile_height, padding, mask_blur, force_uniform_tiles)
     with torch.cuda.device(device):

@@ -14,6 +14,7 @@ import numpy as np
 import torch
 
 from . import _native as nat
+from .casts import reference_f32
 from .lru import LruCache
 from .planner import Plan, Tile, WorkList, get_plan
 
@@ -382,7 +383,7 @@ def denoise_packed(plan: Plan, tile_ids: Sequence[int], buf: torch.Tensor, offs:
         if tuple(res.shape) != tuple(view.shape):
             raise ValueError(f"denoiser returned {tuple(res.shape)}, expected {tuple(view.shape)}")
         _require_cuda(res, "denoiser output")
-        return res.to(torch.float32).contiguous().view(-1)
+        return reference_f32(res).contiguous().view(-1)
     out = torch.empty_like(buf)
     for ids, view in groups:
         res = denoiser(view, [plan.tiles[i] for i in ids])
@@ -390,7 +391,7 @@ def denoise_packed(plan: Plan, tile_ids: Sequence[int], buf: torch.Tensor, offs:
             raise ValueError(f"denoiser returned {tuple(res.shape)}, expected {tuple(view.shape)}")
         _require_cuda(res, "denoiser output")
         o0 = int(offs[list(tile_ids).index(ids[0])])
-        out[o0: o0 + view.numel()].view_as(view).copy_(res.to(torch.float32))
+        out[o0: o0 + view.numel()].view_as(view).copy_(reference_f32(res))
     return out
 
 
@@ -961,7 +962,7 @@ def upscale_host(host_image: torch.Tensor, denoiser: Denoiser, tile_width: int, 
     if host_image.is_cuda:
         raise ValueError("upscale_host takes a host tensor; use upscale_single for device tensors")
     device = device or torch.device("cuda", torch.cuda.current_device())
-    x = host_image.to(torch.float32).contiguous()
+    x = reference_f32(host_image).contiguous()
     B, H, W, _ = x.shape
     plan = get_plan(W, H, tile_width, tile_height, padding, mask_blur, force_uniform_tiles)
     with torch.cuda.device(device):

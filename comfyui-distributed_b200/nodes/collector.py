@@ -14,13 +14,14 @@ import json
 import torch
 
 from .. import dist as usdu_dist
+from ..casts import reference_f32
 
 
 def _native_pack(images: torch.Tensor) -> torch.Tensor:
-    """fp32 [B,H,W,C] (any device) -> u8 CUDA tensor, trunc(255*x) on the GPU."""
+    """IMAGE [B,H,W,C] (any device) -> u8 CUDA tensor, the reference's trunc(255*x) on the GPU."""
     from .. import _native as nat
     dev = images.device if images.is_cuda else torch.device("cuda", torch.cuda.current_device())
-    x = images.to(torch.float32).contiguous()
+    x = reference_f32(images).contiguous()
     if not x.is_cuda:
         x = (x if x.is_pinned() else x.pin_memory()).to(dev, non_blocking=True)
     q = torch.empty(x.shape, dtype=torch.uint8, device=dev)

@@ -22,6 +22,7 @@ import os
 import torch
 
 from .. import dist as usdu_dist
+from ..casts import reference_f32
 from ..denoise import ComfySampler
 from ..engine import upscale_host, upscale_single
 
@@ -142,10 +143,10 @@ class UltimateSDUpscaleDistributed:
             if out is not NotImplemented:
                 return (upscaled_image,) if worker else (out,)
         if upscaled_image.is_cuda:
-            image = upscaled_image.to(torch.float32)
+            image = reference_f32(upscaled_image)
         else:
             # ComfyUI IMAGE tensors live on the host: stage through pinned memory
-            host = upscaled_image.to(torch.float32).contiguous()
+            host = reference_f32(upscaled_image).contiguous()
             host = host if host.is_pinned() else host.pin_memory()
             image = host.to(dev, non_blocking=True)
         _, H, W, _ = image.shape

@@ -133,8 +133,14 @@ def crop_geometry(W: int, H: int, x: int, y: int, tw: int, th: int, padding: int
 # float <-> u8   (utils/image.py:8-18)
 # --------------------------------------------------------------------------------------
 def quantize_u8(x: np.ndarray) -> np.ndarray:
-    """(255 * x).astype(uint8): fp32 multiply then C truncation.  Inputs in [0,1]."""
-    return (np.float32(255) * np.asarray(x, dtype=np.float32)).astype(np.uint8)
+    """(255 * x).astype(uint8) as the reference runs it: the multiply rounds in x's own dtype (fp16, fp32 or fp64;
+    anything else is taken as fp32), then numpy's x86 cast truncates and keeps the low byte.  NaN, +-inf and products
+    outside [-2^31, 2^31) give 0 (tests/test_u8_cast_model.py pins this on the host)."""
+    x = np.asarray(x)
+    if x.dtype not in (np.float16, np.float64):
+        x = x.astype(np.float32)
+    with np.errstate(over="ignore", invalid="ignore"):
+        return (x.dtype.type(255) * x).astype(np.uint8)
 
 
 def dequantize_u8(u: np.ndarray) -> np.ndarray:
