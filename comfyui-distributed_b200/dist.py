@@ -34,6 +34,35 @@ def dist_info(group=None) -> Tuple[int, int]:
     return 0, 1
 
 
+def _parse_worker_index(worker_id: str) -> Optional[int]:
+    """An injected worker id as the reference reads it: "worker_N" or a plain integer N; None when it does not parse
+    (nodes/utilities.py:60-75)."""
+    try:
+        return int(worker_id.split("_")[1]) if worker_id.startswith("worker_") else int(worker_id)
+    except (ValueError, IndexError):
+        return None
+
+
+def participant(is_worker: bool = False, worker_id: str = "", group=None) -> Optional[int]:
+    """Which participant of a distributed prompt this process is: None for the master, k for worker k (0-based, the
+    numbering of the reference's orchestrator, which injects "worker_k" for the k-th enabled worker,
+    prompt_transform.py:327).  The per-participant utility nodes (DistributedSeed, DistributedValue) key off it.
+
+    * No process group (world size 1): the hidden inputs decide, as in the reference -- is_worker=False is the master,
+      is_worker=True is the worker that worker_id names; a worker_id that does not parse falls back to the master.
+    * World size > 1 (SPMD, one rank per GPU): the rank decides, as for UltimateSDUpscaleDistributed.  Rank 0 is the
+      master; rank r >= 1 is worker r - 1 unless an injected worker_id parses, and then that worker.  Without hidden
+      inputs worker k is rank k + 1, the rank order DistributedCollector gathers in; with the orchestrator's ids it is
+      the position in enabled_worker_ids, the order the collector uses then."""
+    rank, world = dist_info(group)
+    if world == 1:
+        return _parse_worker_index(worker_id) if is_worker else None
+    if rank == 0:
+        return None
+    k = _parse_worker_index(worker_id)
+    return rank - 1 if k is None else k
+
+
 # --------------------------------------------------------------------------------------
 # transport (device agnostic: NCCL on CUDA tensors, gloo on CPU tensors in the tests)
 # --------------------------------------------------------------------------------------

@@ -1,14 +1,31 @@
 from .distributed_upscale import UltimateSDUpscaleDistributed
 from .collector import DistributedCollectorNode
-from .utilities import ImageBatchDivider
+from .utilities import (
+    AudioBatchDivider,
+    DistributedEmptyImage,
+    DistributedModelName,
+    DistributedSeed,
+    DistributedValue,
+    ImageBatchDivider,
+)
 
 NODE_CLASS_MAPPINGS = {
     "UltimateSDUpscaleDistributed": UltimateSDUpscaleDistributed,
     "DistributedCollector": DistributedCollectorNode,
+    "DistributedSeed": DistributedSeed,
+    "DistributedModelName": DistributedModelName,
+    "DistributedValue": DistributedValue,
     "ImageBatchDivider": ImageBatchDivider,
+    "AudioBatchDivider": AudioBatchDivider,
+    "DistributedEmptyImage": DistributedEmptyImage,
 }
 NODE_DISPLAY_NAME_MAPPINGS = {
     "UltimateSDUpscaleDistributed": "Ultimate SD Upscale Distributed (No Upscale)",
     "DistributedCollector": "Distributed Collector",
+    "DistributedSeed": "Distributed Seed",
+    "DistributedModelName": "Distributed Model Name",
+    "DistributedValue": "Distributed Value",
     "ImageBatchDivider": "Image Batch Divider",
+    "AudioBatchDivider": "Audio Batch Divider",
+    "DistributedEmptyImage": "Distributed Empty Image",
 }
