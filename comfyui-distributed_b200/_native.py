@@ -16,7 +16,17 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libusdu_b200.so")
 
 # constants mirrored from include/usdu_b200.h (checked against the header in tests)
-ABI_VERSION = 8
+ABI_VERSION = 9
+ERR_INVALID = -1
+CANVAS_SLACK = 16
+PLAN_INFO_WORDS = 16
+(PI_TW, PI_TH, PI_TILES, PI_TAB_WORDS, PI_TABLES, PI_MASK_CLASSES, PI_MASK_POOL_BYTES, PI_FAST, PI_MMA, PI_PATH,
+ PI_NEIGHBOR_WORDS) = range(11)
+PLAN_TILE_WORDS = 12
+PLAN_TABLE_WORDS = 8
+WL_INFO_WORDS = 16
+(WL_ITEMS, WL_ITEM_WORDS, WL_COVER, WL_PATCH_W, WL_PATCH_H, WL_ALGO_BYTES, WL_N_LAUNCH, WL_BLOCK_ROWS, WL_BLOCK_COLS,
+ WL_ROW0, WL_ROW1, WL_PATH, WL_KS2, WL_TOTAL, WL_FLAGS, WL_GRID) = range(16)
 TILE_WORDS = 24
 T_X1, T_Y1, T_EW, T_EH, T_PW, T_PH, T_MASK_OFF, T_MASK_PITCH = range(8)
 T_TAB_CROP_H, T_TAB_CROP_V, T_TAB_BLEND_H, T_TAB_BLEND_V = 8, 9, 10, 11
@@ -89,6 +99,27 @@ _SIGNATURES = {
                                       c_int, c_int, c_int, c_void_p, c_int, c_void_p]),
     "usdu_tile_blend": (c_int, [c_void_p, c_int, c_int, c_int, c_int64, c_void_p, c_void_p, c_void_p, c_void_p,
                                 c_int, c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_void_p]),
+    "usdu_canvas_pitch": (c_int64, [c_int]),
+    "usdu_canvas_bytes": (c_int64, [c_int, c_int, c_int]),
+    "usdu_plan_create": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, POINTER(c_void_p)]),
+    "usdu_plan_destroy": (c_int, [c_void_p]),
+    "usdu_plan_info": (c_int, [c_void_p, POINTER(c_int64)]),
+    "usdu_plan_tiles": (c_int, [c_void_p, POINTER(c_int32)]),
+    "usdu_plan_tile_desc": (c_int, [c_void_p, POINTER(c_int32)]),
+    "usdu_plan_tables": (c_int, [c_void_p, POINTER(c_int32)]),
+    "usdu_plan_table_index": (c_int, [c_void_p, POINTER(c_int32)]),
+    "usdu_plan_mask_specs": (c_int, [c_void_p, POINTER(c_int32)]),
+    "usdu_plan_neighbors": (c_int, [c_void_p, POINTER(c_int32), POINTER(c_int32)]),
+    "usdu_plan_waves": (c_int, [c_void_p, POINTER(c_int32), c_int, POINTER(c_int32)]),
+    "usdu_plan_crop_worklist": (c_int, [c_void_p, POINTER(c_int32), c_int, c_int, c_int, c_int, c_int, c_int,
+                                        POINTER(c_void_p)]),
+    "usdu_plan_blend_worklist": (c_int, [c_void_p, POINTER(c_int32), POINTER(c_int64), c_int, c_int, c_int, c_int, c_int,
+                                         c_int, c_int, POINTER(c_int64), c_int, c_int, c_int, c_int, POINTER(c_void_p)]),
+    "usdu_worklist_destroy": (c_int, [c_void_p]),
+    "usdu_worklist_info": (c_int, [c_void_p, POINTER(c_int64)]),
+    "usdu_worklist_items": (c_int, [c_void_p, POINTER(c_int32)]),
+    "usdu_worklist_cover": (c_int, [c_void_p, POINTER(c_int32)]),
+    "usdu_worklist_slots": (c_int, [c_void_p, POINTER(c_int64)]),
 }
 
 EXPORTS = tuple(_SIGNATURES)
@@ -187,6 +218,131 @@ def box_blur_params(radius: float):
     _check(lib().usdu_box_blur_params(float(radius), ctypes.byref(rad), ctypes.byref(ww), ctypes.byref(fw)),
            "usdu_box_blur_params")
     return rad.value, ww.value, fw.value
+
+
+def canvas_bytes(B: int, H: int, W: int) -> int:
+    n = lib().usdu_canvas_bytes(B, H, W)
+    if n < 0:
+        _check(int(n), "usdu_canvas_bytes")
+    return int(n)
+
+
+# ---- host-side planner (usdu_plan_*) --------------------------------------------------
+def _i64p(a: np.ndarray):
+    assert a.dtype == np.int64 and a.flags["C_CONTIGUOUS"]
+    return a.ctypes.data_as(POINTER(c_int64))
+
+
+def _ids(tile_ids) -> np.ndarray:
+    return np.ascontiguousarray(np.asarray(tile_ids, dtype=np.int64).reshape(-1).astype(np.int32))
+
+
+def _read_worklist(h: c_void_p) -> dict:
+    """Contents of a usdu_worklist handle (destroyed here): info words, items int32 [n, words], cover int32 [m, 4]
+    and the crop's slot offsets int64."""
+    L = lib()
+    try:
+        info = np.zeros(WL_INFO_WORDS, np.int64)
+        _check(L.usdu_worklist_info(h, _i64p(info)), "usdu_worklist_info")
+        items = np.zeros((int(info[WL_ITEMS]), int(info[WL_ITEM_WORDS])), np.int32)
+        if items.size:
+            _check(L.usdu_worklist_items(h, _i32p(items)), "usdu_worklist_items")
+        cover = np.zeros((int(info[WL_COVER]), COVER_WORDS), np.int32)
+        if cover.size:
+            _check(L.usdu_worklist_cover(h, _i32p(cover)), "usdu_worklist_cover")
+        return {"info": info, "items": items, "cover": cover}
+    finally:
+        L.usdu_worklist_destroy(h)
+
+
+class NativePlan:
+    """Owner of one usdu_plan handle: the library's planner for one job geometry (include/usdu_b200.h, planner
+    section).  Inputs the library rejects (a tile size that rounds to zero, feather templates of 2 GiB or more ...)
+    raise ValueError with the library's message."""
+
+    def __init__(self, W: int, H: int, tile_width: int, tile_height: int, padding: int, mask_blur: int, uniform: bool):
+        L = lib()
+        self._lib = L
+        self._h = c_void_p()
+        st = L.usdu_plan_create(W, H, tile_width, tile_height, padding, mask_blur, int(bool(uniform)), ctypes.byref(self._h))
+        if st == ERR_INVALID:
+            raise ValueError(L.usdu_last_error().decode())
+        _check(st, "usdu_plan_create")
+        self.info = np.zeros(PLAN_INFO_WORDS, np.int64)
+        _check(L.usdu_plan_info(self._h, _i64p(self.info)), "usdu_plan_info")
+
+    def __del__(self):
+        h = getattr(self, "_h", None)
+        if h:
+            self._lib.usdu_plan_destroy(h)
+            self._h = None
+
+    def _array(self, fn: str, shape) -> np.ndarray:
+        a = np.zeros(shape, np.int32)
+        if a.size:
+            _check(getattr(self._lib, fn)(self._h, _i32p(a)), fn)
+        return a
+
+    def tiles(self) -> np.ndarray:
+        return self._array("usdu_plan_tiles", (int(self.info[PI_TILES]), PLAN_TILE_WORDS))
+
+    def tile_desc(self) -> np.ndarray:
+        return self._array("usdu_plan_tile_desc", (int(self.info[PI_TILES]), TILE_WORDS))
+
+    def tables(self) -> np.ndarray:
+        return self._array("usdu_plan_tables", int(self.info[PI_TAB_WORDS]))
+
+    def table_index(self) -> np.ndarray:
+        return self._array("usdu_plan_table_index", (int(self.info[PI_TABLES]), PLAN_TABLE_WORDS))
+
+    def mask_specs(self) -> np.ndarray:
+        return self._array("usdu_plan_mask_specs", (int(self.info[PI_MASK_CLASSES]), MASK_WORDS))
+
+    def neighbors(self):
+        T = int(self.info[PI_TILES])
+        first = np.zeros(T + 1, np.int32)
+        lst = np.zeros(max(int(self.info[PI_NEIGHBOR_WORDS]), 1), np.int32)
+        _check(self._lib.usdu_plan_neighbors(self._h, _i32p(first), _i32p(lst)), "usdu_plan_neighbors")
+        return [lst[first[i]:first[i + 1]].tolist() for i in range(T)]
+
+    def waves(self, order) -> np.ndarray:
+        """Level of every entry of `order` (usdu_plan_waves)."""
+        ids = _ids(order)
+        level = np.zeros(max(ids.size, 1), np.int32)
+        st = self._lib.usdu_plan_waves(self._h, _i32p(ids), ids.size, _i32p(level))
+        if st == ERR_INVALID:
+            raise ValueError(self._lib.usdu_last_error().decode())
+        _check(min(st, 0), "usdu_plan_waves")
+        return level[:ids.size]
+
+    def crop_worklist(self, tile_ids, B: int, path: int, share: int, sm_count: int, mma_block_rows: int) -> dict:
+        ids = _ids(tile_ids)
+        h = c_void_p()
+        _check(self._lib.usdu_plan_crop_worklist(self._h, _i32p(ids), ids.size, B, path, share, sm_count, mma_block_rows,
+                                                 ctypes.byref(h)), "usdu_plan_crop_worklist")
+        slots = np.zeros(max(ids.size, 1), np.int64)
+        if ids.size:
+            _check(self._lib.usdu_worklist_slots(h, _i64p(slots)), "usdu_worklist_slots")
+        out = _read_worklist(h)
+        out["slots"] = slots[:ids.size]
+        return out
+
+    def blend_worklist(self, tile_ids, offs, src_bytes: int, B: int, path: int, part, share: int, rects, keep: int,
+                       sm_count: int, mma_block_rows: int) -> dict:
+        """part = (i, n) or None; rects int64 [m, 4] with keep 1 / 0, or keep = -1 for every block."""
+        ids = _ids(tile_ids)
+        offs = np.ascontiguousarray(np.asarray(offs, dtype=np.int64).reshape(-1))
+        if offs.size < ids.size:
+            raise ValueError(f"blend work list: {offs.size} source offsets for {ids.size} tiles")
+        offs = np.ascontiguousarray(offs[:max(ids.size, 1)]) if offs.size else np.zeros(1, np.int64)
+        rects = np.zeros((0, 4), np.int64) if rects is None else np.asarray(rects, dtype=np.int64).reshape(-1, 4)
+        rbuf = np.ascontiguousarray(rects if rects.size else np.zeros((1, 4), np.int64))
+        pi, pn = part if part is not None else (0, 0)
+        h = c_void_p()
+        _check(self._lib.usdu_plan_blend_worklist(self._h, _i32p(ids), _i64p(offs), ids.size, src_bytes, B, path, pi, pn, share,
+                                                  _i64p(rbuf), rects.shape[0], keep, sm_count, mma_block_rows, ctypes.byref(h)),
+               "usdu_plan_blend_worklist")
+        return _read_worklist(h)
 
 
 # ---- device entry points (raw pointers; torch supplies memory and the stream) ----------

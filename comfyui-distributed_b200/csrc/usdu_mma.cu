@@ -11,7 +11,7 @@
 // warpgroup per 64 output rows; the patches here are 16-row M-tiles of 1 or 2 k-steps, so the warp-level IMMA stays.
 //
 // Both passes put the COEFFICIENTS in the A operand (16 outputs x 32 inputs, built on the host in fragment order:
-// planner.build_mma_frags) and the PIXELS in B:
+// build_mma_frags in usdu_plan.cpp) and the PIXELS in B:
 //   H pass  M = 16 output pixels of one channel, N = 8 rows, K = 32 input pixels.  Input staged PLANAR (one byte
 //           plane per channel), so a B register is 4 consecutive pixels of a row: one aligned LDS.32.
 //   V pass  M = 16 output rows, N = 8 byte columns, K = 32 input rows.  The H pass leaves its u8 results ROW-PACKED,
@@ -75,7 +75,7 @@ __device__ __forceinline__ uint32_t pack2(int lo, int hi, uint32_t upper) {
     return d;
 }
 
-// fragment section of a table (planner.build_mma_frags): {n_mt, ksteps, 0, 0} then per M-tile {k0, 0, 0, 0, fragments of
+// fragment section of a table (usdu_plan.cpp build_mma_frags): {n_mt, ksteps, 0, 0} then per M-tile {k0, 0, 0, 0, fragments of
 // (k-step, limb): 32 lanes x 4 registers}.  Everything is addressed from (section, mt, KS): no dependent load in front of
 // the fragment loads.
 struct FragTable {

@@ -16,8 +16,11 @@
  *   upscale/tile_ops.py:289-308        create_tile_mask (rectangle + GaussianBlur)
  *   upscale/tile_ops.py:310-349        blend_tile (LANCZOS back + alpha composite)
  *   upscale/worker_comms.py:16-108     tile payload packing (PNG) -> usdu_pack_tiles_u8
- * The geometry (upscale/tile_ops.py:14-32, utils/usdu_utils.py:49-112) stays on the host
- * in Python, like the reference; it produces the descriptor arrays documented below.
+ * The geometry (upscale/tile_ops.py:14-32, utils/usdu_utils.py:49-112) runs on the host, like
+ * the reference, inside this library: the planner section at the end (usdu_plan_create ...)
+ * builds the tile geometry, the descriptor and table arrays documented below, the dependency
+ * waves and the work lists of every kernel, so a C/C++ host drives the whole tile path
+ * without Python (csrc/tools/usdu_c_job.c is a complete single-GPU job).
  */
 #ifndef USDU_B200_H
 #define USDU_B200_H
@@ -32,7 +35,7 @@ extern "C" {
 #pragma GCC visibility push(default) /* the library itself is built with -fvisibility=hidden */
 #endif
 
-#define USDU_ABI_VERSION 8
+#define USDU_ABI_VERSION 9
 
 typedef enum usdu_status {
     USDU_OK = 0,
@@ -191,7 +194,7 @@ int usdu_box_blur_params(float radius, int32_t* rad, uint32_t* ww, uint32_t* fw)
 #define USDU_FLAG_FAST 1
 /* USDU_FLAG_MMA selects the tensor-core kernels (usdu_mma.cu: every LANCZOS tap runs as mma.sync.m16n8k32 on 8-bit
  * coefficient limbs, bit-identical results).  items_dev then holds job records in the TENSOR-CORE flavour: the same 32
- * words, with USDU_J_ROWS_H / _V = table-pool index of the axis' fragment section (host side: planner.build_mma_frags;
+ * words, with USDU_J_ROWS_H / _V = table-pool index of the axis' fragment section (built by usdu_plan_create;
  * {n_mtiles, ksteps, 0, 0} then per M-tile {k0, 0, 0, 0, per (k-step, limb) 32 lanes x 4 registers}),
  * USDU_J_TAPS_H / _V = k-steps (1 or 2), USDU_J_IX0 / _IY0 = first staged input column / row (multiples of 4),
  * USDU_J_COLS a multiple of 4, USDU_J_LEAD = 0, crop: USDU_J_SRC_A a multiple of 4 and USDU_J_CY1 = block rows (16 / 32).
@@ -217,7 +220,15 @@ int usdu_box_blur_params(float radius, int32_t* rad, uint32_t* ww, uint32_t* fw)
  * (usdu_gather_dequantize), so nothing in the package sets this flag any more. */
 #define USDU_FLAG_REMOTE_CANVAS (1 << 24)
 /* Q0: canvas_u8[b][y][x*3+c] = (uint8)(255.f * img[b][y][x][c])   (utils/image.py:8-10)
- * pitch = bytes per canvas row (>= 3*W, multiple of 16); frame stride = H*pitch. */
+ * pitch = bytes per canvas row (>= 3*W, multiple of 16); frame stride = H*pitch.
+ * The allocation behind a canvas must hold USDU_CANVAS_SLACK bytes more than B*H*pitch: the staging of the
+ * integer-pipe kernels reads whole 12-byte chunks and, for widths that are not multiples of 4, may touch up to 4
+ * bytes past the last row's pitch (the values are discarded).  usdu_canvas_bytes() gives the size to allocate. */
+#define USDU_CANVAS_SLACK 16
+/* bytes per canvas row the package uses: 3*W rounded up to 128 */
+int64_t usdu_canvas_pitch(int W);
+/* B*H*usdu_canvas_pitch(W) + USDU_CANVAS_SLACK */
+int64_t usdu_canvas_bytes(int B, int H, int W);
 int usdu_quantize_canvas(const float* img_dev, uint8_t* canvas_dev, int B, int H, int W,
                          int64_t pitch, void* stream);
 /* canvas u8 -> fp32 image (u / 255.0f, utils/image.py:12-14) */
@@ -330,6 +341,98 @@ int usdu_plane_resample_u8(const uint8_t* src_dev, int n, int src_h, int src_w, 
 int usdu_plane_pad_fill_u8(const uint8_t* src_dev, int n, int h, int w, int64_t src_pitch, int64_t src_plane,
                            int hp, int vp, const int32_t* row_index_dev, const int32_t* col_index_dev,
                            uint8_t* dst_dev, int64_t dst_pitch, int64_t dst_plane, void* stream);
+
+/* ---- host-side planner (no device needed) -------------------------------------------------
+ * A plan is one job geometry: usdu_plan_create(W, H, tile_width, tile_height, padding, mask_blur,
+ * uniform) applies round_to_multiple (ties to even, upscale/tile_ops.py:14-16), calculate_tiles
+ * (:18-32), the crop window and expand_crop (utils/usdu_utils.py:49-112) and, for uniform = 0,
+ * the multiple-of-8 target size; then it builds the table pool (tables of every crop and blend
+ * axis, each followed by its tensor-core fragment section while the plan qualifies for the
+ * tensor-core kernels; every section starts at a multiple of 4 int32), the feather-mask specs,
+ * the tile descriptors and the overlap graph.  A tile size that rounds to zero, an empty canvas
+ * and feather templates of 2 GiB or more are rejected with USDU_ERR_INVALID.  The plan is
+ * immutable; the query calls copy into caller-allocated arrays sized from usdu_plan_info. */
+typedef struct usdu_plan usdu_plan;
+int usdu_plan_create(int W, int H, int tile_width, int tile_height, int padding, int mask_blur, int uniform,
+                     usdu_plan** plan);
+int usdu_plan_destroy(usdu_plan* plan);
+#define USDU_PLAN_INFO_WORDS 16    /* int64 words of usdu_plan_info */
+#define USDU_PI_TW 0               /* tile size after round_to_multiple */
+#define USDU_PI_TH 1
+#define USDU_PI_TILES 2            /* tile positions (row-major grid) */
+#define USDU_PI_TAB_WORDS 3        /* int32 words of the table pool */
+#define USDU_PI_TABLES 4           /* resample tables in the pool (rows of usdu_plan_table_index) */
+#define USDU_PI_MASK_CLASSES 5     /* feather-mask specs (rows of usdu_plan_mask_specs) */
+#define USDU_PI_MASK_POOL_BYTES 6  /* bytes of the mask pool usdu_build_feather_masks fills */
+#define USDU_PI_FAST 7             /* 1: every table has packed rows (integer-pipe kernels usable) */
+#define USDU_PI_MMA 8              /* 1: ... and tensor-core fragments, windows on 4-pixel columns */
+#define USDU_PI_PATH 9             /* best kernel path: 0 generic, 1 integer-pipe (USDU_FLAG_FAST), 2 tensor-core */
+#define USDU_PI_NEIGHBOR_WORDS 10  /* entries of usdu_plan_neighbors' list */
+int usdu_plan_info(const usdu_plan* plan, int64_t* info);
+/* per tile USDU_PLAN_TILE_WORDS int32: {x, y} grid origin, {x1, y1} crop window origin, {ew, eh} window size,
+ * {pw, ph} processing size, {bx2, by2} exclusive far corner of the clipped mask rectangle (which starts at x, y),
+ * feather-mask class, 0 */
+#define USDU_PLAN_TILE_WORDS 12
+int usdu_plan_tiles(const usdu_plan* plan, int32_t* tiles);
+/* tiles x USDU_TILE_WORDS descriptors (upload for the tile kernels) */
+int usdu_plan_tile_desc(const usdu_plan* plan, int32_t* desc);
+/* the table pool, USDU_PI_TAB_WORDS int32 (upload for the tile kernels) */
+int usdu_plan_tables(const usdu_plan* plan, int32_t* pool);
+/* per table USDU_PLAN_TABLE_WORDS int32: {in size, out size, pool offset, pool index of packed row 0, pool index of
+ * the fragment section (-1 = none), k-steps, staged taps of the integer-pipe kernels, taps the job records carry} */
+#define USDU_PLAN_TABLE_WORDS 8
+int usdu_plan_table_index(const usdu_plan* plan, int32_t* index);
+/* USDU_PI_MASK_CLASSES x USDU_MASK_WORDS specs for usdu_mask_scratch_bytes / usdu_build_feather_masks */
+int usdu_plan_mask_specs(const usdu_plan* plan, int32_t* specs);
+/* tiles whose crop windows intersect: tile i's list is list[first[i] .. first[i+1]); first has tiles + 1 entries */
+int usdu_plan_neighbors(const usdu_plan* plan, int32_t* first, int32_t* list);
+/* Level schedule of the tiles order[0..n) (distinct ids) under progressive semantics (upscale/modes/single_gpu.py:40-64):
+ * wave[i] = level of order[i]; tiles of one level have disjoint windows and run as one crop / sampler / blend step,
+ * levels in ascending order.  Returns the number of levels, or a negative usdu_status. */
+int usdu_plan_waves(const usdu_plan* plan, const int32_t* order, int n, int32_t* wave);
+
+/* Work lists: one kernel launch each, built for
+ *   path: 0 generic kernels, 1 integer-pipe (USDU_FLAG_FAST), 2 tensor-core (USDU_FLAG_MMA); lowered to what the plan
+ *         supports (USDU_WL_PATH tells which);
+ *   share: launches expected to run side by side (each gets 1/share of the machine in the block-height model);
+ *   sm_count: SMs of the block-height model, 0 = query the current device (132 when there is none);
+ *   mma_block_rows: tensor-core block height to force (16 or 32), 0 = the model's choice.
+ * Crop: the tiles' [B][PH][PW][3] fp32 outputs are packed in list order (usdu_worklist_slots: element offset per tile,
+ * USDU_WL_TOTAL elements in all).  Blend: src_offsets[i] = element offset of tile_ids[i]'s processed block in the
+ * source, src_bytes = 4 (fp32) or 1 (u8); the list order is the blend order.  part_n > 0 restricts the launch to the
+ * part_i-th of part_n horizontal slabs of canvas block rows (USDU_WL_ROW0 / _ROW1); select_keep = 1 / 0 keeps only the
+ * canvas blocks that meet one / none of the n_rects rectangles {x0, y0, x1, y1} (int64), -1 = all blocks.
+ * Launch: items = usdu_worklist_items, grid = USDU_WL_GRID, flags = USDU_WL_FLAGS, patch = USDU_WL_PATCH_W / _H, and for
+ * the generic blend cover_dev = usdu_worklist_cover. */
+typedef struct usdu_worklist usdu_worklist;
+int usdu_plan_crop_worklist(const usdu_plan* plan, const int32_t* tile_ids, int n, int B, int path, int share,
+                            int sm_count, int mma_block_rows, usdu_worklist** wl);
+int usdu_plan_blend_worklist(const usdu_plan* plan, const int32_t* tile_ids, const int64_t* src_offsets, int n,
+                             int src_bytes, int B, int path, int part_i, int part_n, int share,
+                             const int64_t* select_rects, int n_rects, int select_keep, int sm_count,
+                             int mma_block_rows, usdu_worklist** wl);
+int usdu_worklist_destroy(usdu_worklist* wl);
+#define USDU_WL_INFO_WORDS 16      /* int64 words of usdu_worklist_info */
+#define USDU_WL_ITEMS 0            /* rows of usdu_worklist_items */
+#define USDU_WL_ITEM_WORDS 1       /* int32 per row: USDU_JOB_WORDS, USDU_CROP_ITEM_WORDS or USDU_BLEND_ITEM_WORDS */
+#define USDU_WL_COVER 2            /* rows (USDU_COVER_WORDS) of usdu_worklist_cover (generic blend) */
+#define USDU_WL_PATCH_W 3
+#define USDU_WL_PATCH_H 4
+#define USDU_WL_ALGO_BYTES 5       /* algorithmic HBM bytes of the launch per frame */
+#define USDU_WL_N_LAUNCH 6         /* blend job records: chain heads (the grid); -1 = one CTA per row */
+#define USDU_WL_BLOCK_ROWS 7
+#define USDU_WL_BLOCK_COLS 8
+#define USDU_WL_ROW0 9             /* part_n > 0: canvas rows [ROW0, ROW1) of the slab; else -1 */
+#define USDU_WL_ROW1 10
+#define USDU_WL_PATH 11
+#define USDU_WL_KS2 12             /* tensor-core records with a two-k-step axis (set USDU_FLAG_MMA_KS2) */
+#define USDU_WL_TOTAL 13           /* crop: fp32 elements of the packed output */
+#define USDU_WL_FLAGS 14           /* the `flags` argument of the launch */
+#define USDU_WL_GRID 15            /* the `n_items` argument of the launch */
+int usdu_worklist_info(const usdu_worklist* wl, int64_t* info);
+int usdu_worklist_items(const usdu_worklist* wl, int32_t* items);
+int usdu_worklist_cover(const usdu_worklist* wl, int32_t* cover);
+int usdu_worklist_slots(const usdu_worklist* wl, int64_t* offsets);
 
 #if defined(__GNUC__)
 #pragma GCC visibility pop
