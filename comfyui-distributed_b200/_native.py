@@ -16,7 +16,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libusdu_b200.so")
 
 # constants mirrored from include/usdu_b200.h (checked against the header in tests)
-ABI_VERSION = 9
+ABI_VERSION = 10
 ERR_INVALID = -1
 CANVAS_SLACK = 16
 PLAN_INFO_WORDS = 16
@@ -85,6 +85,12 @@ _SIGNATURES = {
     "usdu_tile_crop_resize_f32": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p]),
     "usdu_quantize_rows": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int64, c_int, c_int, c_void_p]),
     "usdu_dequantize_rows": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int64, c_int, c_int, c_void_p]),
+    "usdu_stream_args_set": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
+    "usdu_quantize_rows_streamed": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int64, c_int, c_int, c_int, c_void_p]),
+    "usdu_dequantize_rows_streamed": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int64, c_int, c_int, c_int, c_void_p]),
+    "usdu_graph_instantiate": (c_int, [c_void_p, c_int, POINTER(c_void_p)]),
+    "usdu_graph_launch": (c_int, [c_void_p, c_void_p]),
+    "usdu_graph_exec_destroy": (c_int, [c_void_p]),
     "usdu_pack_tiles_u8": (c_int, [c_void_p, c_void_p, c_int64, c_void_p]),
     "usdu_unpack_tiles_f32": (c_int, [c_void_p, c_void_p, c_int64, c_void_p]),
     "usdu_t0_denoise": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_float, c_void_p]),
@@ -356,6 +362,38 @@ def quantize_rows(img_ptr, canvas_ptr, B, H, W, pitch, y0, y1, stream):
 
 def dequantize_rows(canvas_ptr, img_ptr, B, H, W, pitch, y0, y1, stream):
     _check(lib().usdu_dequantize_rows(canvas_ptr, img_ptr, B, H, W, pitch, y0, y1, stream), "usdu_dequantize_rows")
+
+
+STREAM_ARGS_BYTES = 16          # sizeof(usdu_stream_args): the fp32 image and result addresses
+
+
+def stream_args_set(args_ptr, img_ptr, out_ptr, stream):
+    _check(lib().usdu_stream_args_set(args_ptr, img_ptr, out_ptr, stream), "usdu_stream_args_set")
+
+
+def quantize_rows_streamed(args_ptr, canvas_ptr, B, H, W, pitch, y0, y1, max_ctas, stream):
+    _check(lib().usdu_quantize_rows_streamed(args_ptr, canvas_ptr, B, H, W, pitch, y0, y1, max_ctas, stream),
+           "usdu_quantize_rows_streamed")
+
+
+def dequantize_rows_streamed(canvas_ptr, args_ptr, B, H, W, pitch, y0, y1, max_ctas, stream):
+    _check(lib().usdu_dequantize_rows_streamed(canvas_ptr, args_ptr, B, H, W, pitch, y0, y1, max_ctas, stream),
+           "usdu_dequantize_rows_streamed")
+
+
+def graph_instantiate(graph_handle: int, high_priority: bool) -> int:
+    """cudaGraphExec_t (as an int) of a captured cudaGraph_t; see usdu_graph_instantiate."""
+    h = c_void_p()
+    _check(lib().usdu_graph_instantiate(graph_handle, int(bool(high_priority)), ctypes.byref(h)), "usdu_graph_instantiate")
+    return int(h.value)
+
+
+def graph_launch(exec_handle: int, stream):
+    _check(lib().usdu_graph_launch(exec_handle, stream), "usdu_graph_launch")
+
+
+def graph_exec_destroy(exec_handle: int):
+    _check(lib().usdu_graph_exec_destroy(exec_handle), "usdu_graph_exec_destroy")
 
 
 def gather_dequantize(slab_ptrs, slab_rows, img_ptr, B, H, W, pitch, stream):

@@ -15,9 +15,9 @@ namespace usdu {
 // Q0 / dequantise / Q1
 // ======================================================================================
 // One thread produces 16 canvas bytes (one uint4 store) from 16 floats (4 x float4 loads).
-__global__ void __launch_bounds__(kThreads)
-quantize_canvas_kernel(const float* __restrict__ img, uint8_t* __restrict__ canvas, int rows, int W3,
-                       int64_t pitch, int vec_ok, int H, int y0, int n_rows) {
+__device__ __forceinline__ void
+quantize_rows_body(const float* __restrict__ img, uint8_t* __restrict__ canvas, int rows, int W3,
+                   int64_t pitch, int vec_ok, int H, int y0, int n_rows) {
     // logical row i of `rows` = B * n_rows  ->  physical row b * H + y0 + (i % n_rows)
     const int chunks = (W3 + 15) >> 4;
     const int64_t total = (int64_t)rows * chunks;
@@ -45,12 +45,18 @@ quantize_canvas_kernel(const float* __restrict__ img, uint8_t* __restrict__ canv
     }
 }
 
+__global__ void __launch_bounds__(kThreads)
+quantize_canvas_kernel(const float* __restrict__ img, uint8_t* __restrict__ canvas, int rows, int W3,
+                       int64_t pitch, int vec_ok, int H, int y0, int n_rows) {
+    quantize_rows_body(img, canvas, rows, W3, pitch, vec_ok, H, y0, n_rows);
+}
+
 // One thread turns ONE canvas word (4 bytes) into one float4: consecutive lanes read consecutive
 // words (128 B per warp load) and write consecutive float4 (512 B per warp store, every 32-byte
 // sector written whole by one instruction).  Rows on blockIdx.y, no integer division.
-__global__ void __launch_bounds__(kThreads)
-dequantize_canvas_kernel(const uint8_t* __restrict__ canvas, float* __restrict__ img, int rows, int W3,
-                         int64_t pitch, int vec_ok, int H, int y0, int n_rows) {
+__device__ __forceinline__ void
+dequantize_rows_body(const uint8_t* __restrict__ canvas, float* __restrict__ img, int rows, int W3,
+                     int64_t pitch, int vec_ok, int H, int y0, int n_rows) {
     if (vec_ok) {
         const int words = W3 >> 2;
         for (int lrow = blockIdx.y; lrow < rows; lrow += gridDim.y) {
@@ -78,6 +84,28 @@ dequantize_canvas_kernel(const uint8_t* __restrict__ canvas, float* __restrict__
         float* dst = img + row * W3;
         for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < W3; j += gridDim.x * blockDim.x) dst[j] = dequant_u8_fast(src[j]);
     }
+}
+
+__global__ void __launch_bounds__(kThreads)
+dequantize_canvas_kernel(const uint8_t* __restrict__ canvas, float* __restrict__ img, int rows, int W3,
+                         int64_t pitch, int vec_ok, int H, int y0, int n_rows) {
+    dequantize_rows_body(canvas, img, rows, W3, pitch, vec_ok, H, y0, n_rows);
+}
+
+// The same two passes for a captured graph that runs them in row bands beside the wave loop (engine.run_split): the fp32
+// image / result address comes from a device-side usdu_stream_args block the host rewrites before every replay, and the
+// grid is a few persistent CTAs that stride over the band, so the pass holds few of the CTA slots the wave kernels need.
+// Both are launched only for 16-byte aligned pointers and widths that are multiples of 4 (the vector path).
+__global__ void __launch_bounds__(kThreads)
+quantize_rows_streamed_kernel(const usdu_stream_args* __restrict__ args, uint8_t* __restrict__ canvas, int rows, int W3,
+                              int64_t pitch, int H, int y0, int n_rows) {
+    quantize_rows_body(args->img_dev, canvas, rows, W3, pitch, 1, H, y0, n_rows);
+}
+
+__global__ void __launch_bounds__(kThreads)
+dequantize_rows_streamed_kernel(const uint8_t* __restrict__ canvas, const usdu_stream_args* __restrict__ args, int rows, int W3,
+                                int64_t pitch, int H, int y0, int n_rows) {
+    dequantize_rows_body(canvas, args->out_dev, rows, W3, pitch, 1, H, y0, n_rows);
 }
 
 // The master's gather of a multi-GPU job: canvas rows [y[q], y[q+1]) come from slab q's canvas (base[q] -- a peer's HBM
@@ -535,8 +563,8 @@ int usdu_quantize_rows(const float* img_dev, uint8_t* canvas_dev, int B, int H, 
     const int W3 = W * 3;
     const int vec_ok = (W3 % 4 == 0) && (((uintptr_t)img_dev & 15) == 0) && (((uintptr_t)canvas_dev & 15) == 0);
     const int64_t total = (int64_t)B * (y1 - y0) * ((W3 + 15) / 16);
-    // short-lived CTAs (up to 128 per SM, ~1 trip each on the 8K canvas): when this pass runs on a side stream beside
-    // small tile waves (engine.OverlappedJob) SM slots turn over every microsecond instead of being held for the whole pass
+    // short-lived CTAs (up to 128 per SM, ~1 trip each on the 8K canvas); the pass that runs beside the wave kernels is
+    // usdu_quantize_rows_streamed, with a few persistent CTAs instead
     const int64_t qblocks = (total + kThreads - 1) / kThreads;
     const int64_t qcap = (int64_t)grid_sms() * 128;
     const int grid = (int)(qblocks < 1 ? 1 : (qblocks > qcap ? qcap : qblocks));
@@ -570,6 +598,102 @@ int usdu_dequantize_rows(const uint8_t* canvas_dev, float* img_dev, int B, int H
     if (gy < 1) gy = 1;
     dequantize_canvas_kernel<<<dim3(gx, (unsigned)gy), kThreads, 0, (cudaStream_t)stream>>>(canvas_dev, img_dev, B * (y1 - y0), W3, pitch, vec_ok, H, y0, y1 - y0);
     USDU_CUDA(cudaGetLastError());
+    return USDU_OK;
+}
+
+int usdu_stream_args_set(usdu_stream_args* args_dev, const float* img_dev, float* out_dev, void* stream) {
+    USDU_REQUIRE(args_dev && img_dev && out_dev, "usdu_stream_args_set: null pointer");
+    USDU_REQUIRE((((uintptr_t)args_dev | (uintptr_t)img_dev | (uintptr_t)out_dev) & 15) == 0,
+                 "usdu_stream_args_set: the block, the image and the result must be 16-byte aligned");
+    const usdu_stream_args host = {img_dev, out_dev};    // pageable: the driver stages it before cudaMemcpyAsync returns
+    USDU_CUDA(cudaMemcpyAsync(args_dev, &host, sizeof(host), cudaMemcpyHostToDevice, (cudaStream_t)stream));
+    return USDU_OK;
+}
+
+// Grid of a streamed pass: at most max_ctas CTAs, each a persistent grid-stride loop over the band.
+static int check_streamed(const char* what, const void* args_dev, const uint8_t* canvas_dev, int B, int H, int W, int64_t pitch,
+                          int y0, int y1, int max_ctas) {
+    USDU_REQUIRE(args_dev && canvas_dev, "%s: null pointer", what);
+    USDU_REQUIRE(B > 0 && H > 0 && W > 0 && W % 4 == 0, "%s: bad shape %dx%dx%d (W must be a multiple of 4)", what, B, H, W);
+    USDU_REQUIRE(0 <= y0 && y0 <= y1 && y1 <= H, "%s: bad row range [%d, %d) of %d", what, y0, y1, H);
+    USDU_REQUIRE(pitch >= 3LL * W && pitch % 16 == 0 && ((uintptr_t)canvas_dev & 15) == 0 && ((uintptr_t)args_dev & 15) == 0,
+                 "%s: pitch %lld must be >= 3*W and a multiple of 16, canvas and argument block 16-byte aligned", what, (long long)pitch);
+    USDU_REQUIRE(max_ctas >= 1, "%s: max_ctas must be >= 1, got %d", what, max_ctas);
+    return USDU_OK;
+}
+
+int usdu_quantize_rows_streamed(const usdu_stream_args* args_dev, uint8_t* canvas_dev, int B, int H, int W, int64_t pitch,
+                                int y0, int y1, int max_ctas, void* stream) {
+    const int s = check_streamed("usdu_quantize_rows_streamed", args_dev, canvas_dev, B, H, W, pitch, y0, y1, max_ctas);
+    if (s != USDU_OK || y1 == y0) return s;
+    const int W3 = W * 3;
+    const int64_t blocks = ((int64_t)B * (y1 - y0) * ((W3 + 15) / 16) + kThreads - 1) / kThreads;
+    const int grid = (int)(blocks < max_ctas ? blocks : max_ctas);
+    quantize_rows_streamed_kernel<<<grid, kThreads, 0, (cudaStream_t)stream>>>(args_dev, canvas_dev, B * (y1 - y0), W3, pitch, H, y0, y1 - y0);
+    USDU_CUDA(cudaGetLastError());
+    return USDU_OK;
+}
+
+int usdu_dequantize_rows_streamed(const uint8_t* canvas_dev, const usdu_stream_args* args_dev, int B, int H, int W,
+                                  int64_t pitch, int y0, int y1, int max_ctas, void* stream) {
+    const int s = check_streamed("usdu_dequantize_rows_streamed", args_dev, canvas_dev, B, H, W, pitch, y0, y1, max_ctas);
+    if (s != USDU_OK || y1 == y0) return s;
+    const int W3 = W * 3;
+    int gx = (W3 / 4 + kThreads * 4 - 1) / (kThreads * 4);          // ~4 words per thread along a row, as usdu_dequantize_rows
+    if (gx > max_ctas) gx = max_ctas;
+    int64_t gy = max_ctas / gx;
+    const int64_t rows = (int64_t)B * (y1 - y0);
+    if (gy > rows) gy = rows;
+    if (gy > 65535) gy = 65535;
+    dequantize_rows_streamed_kernel<<<dim3(gx, (unsigned)gy), kThreads, 0, (cudaStream_t)stream>>>(canvas_dev, args_dev, (int)rows, W3,
+                                                                                                    pitch, H, y0, y1 - y0);
+    USDU_CUDA(cudaGetLastError());
+    return USDU_OK;
+}
+
+int usdu_graph_instantiate(void* graph, int high_priority, void** exec_out) {
+    USDU_REQUIRE(graph && exec_out, "usdu_graph_instantiate: null pointer");
+    cudaGraph_t g = (cudaGraph_t)graph;
+    if (high_priority) {
+        int least = 0, greatest = 0;
+        USDU_CUDA(cudaDeviceGetStreamPriorityRange(&least, &greatest));
+        size_t n = 0;
+        USDU_CUDA(cudaGraphGetNodes(g, nullptr, &n));
+        cudaGraphNode_t* nodes = (cudaGraphNode_t*)malloc((n ? n : 1) * sizeof(cudaGraphNode_t));
+        USDU_REQUIRE(nodes != nullptr, "usdu_graph_instantiate: out of host memory");
+        cudaError_t e = cudaGraphGetNodes(g, nodes, &n);
+        for (size_t i = 0; e == cudaSuccess && i < n; ++i) {
+            cudaGraphNodeType type;
+            e = cudaGraphNodeGetType(nodes[i], &type);
+            if (e != cudaSuccess || type != cudaGraphNodeTypeKernel) continue;
+            cudaKernelNodeParams p = {};
+            // a node the runtime cannot describe (a driver-API launch) is not one of the streamed casts
+            if (cudaGraphKernelNodeGetParams(nodes[i], &p) != cudaSuccess) {
+                (void)cudaGetLastError();
+                p.func = nullptr;
+            }
+            if (p.func == (void*)quantize_rows_streamed_kernel || p.func == (void*)dequantize_rows_streamed_kernel) continue;
+            cudaLaunchAttributeValue v = {};
+            v.priority = greatest;
+            e = cudaGraphKernelNodeSetAttribute(nodes[i], cudaLaunchAttributePriority, &v);
+        }
+        free(nodes);
+        USDU_CUDA(e);
+    }
+    cudaGraphExec_t exec = nullptr;
+    USDU_CUDA(cudaGraphInstantiateWithFlags(&exec, g, high_priority ? cudaGraphInstantiateFlagUseNodePriority : 0));
+    *exec_out = (void*)exec;
+    return USDU_OK;
+}
+
+int usdu_graph_launch(void* exec, void* stream) {
+    USDU_REQUIRE(exec, "usdu_graph_launch: null graph");
+    USDU_CUDA(cudaGraphLaunch((cudaGraphExec_t)exec, (cudaStream_t)stream));
+    return USDU_OK;
+}
+
+int usdu_graph_exec_destroy(void* exec) {
+    if (exec) USDU_CUDA(cudaGraphExecDestroy((cudaGraphExec_t)exec));
     return USDU_OK;
 }
 

@@ -523,13 +523,93 @@ def run_dag(canvas: Canvas, order: Sequence[int], denoiser: Denoiser, lanes: Lis
         main.wait_stream(lanes[ln])
 
 
+# The canvas quantise / dequantise of a graphed 1-GPU job as row bands inside the wave graph (CastBands, run_split), beside
+# the waves that do not touch those rows.  USDU_STREAM_OVERLAP=0 keeps the two eager whole-canvas passes around the graph.
+# USDU_STREAM_CTAS: CTAs of a band beside the waves; USDU_STREAM_BANDS: bands per pass; USDU_STREAM_PRIORITY=1: the wave
+# kernels outrank the bands in CTA dispatch (usdu_graph_instantiate).  Defaults from the sweep in DESIGN section 9.2.
+STREAM_OVERLAP = os.environ.get("USDU_STREAM_OVERLAP", "1") == "1"
+STREAM_CTAS = int(os.environ.get("USDU_STREAM_CTAS", "264"))
+STREAM_BANDS = int(os.environ.get("USDU_STREAM_BANDS", "16"))
+STREAM_PRIORITY = os.environ.get("USDU_STREAM_PRIORITY", "1") == "1"
+
+
+class CastBands:
+    """The quantise and dequantise passes of one graphed job, cut into row bands (Plan.stream_bands) that run on a
+    streaming side stream of the wave graph: every quantise band is enqueued at the start and a stream waits for it just
+    before the first crop that reads its rows; a dequantise band forks after the blend of the last wave that writes its
+    rows.  The first quantise band and the last dequantise band have nothing beside them and run on the whole machine;
+    the others use at most `max_ctas` CTAs.  The fp32 image and result addresses live in a device-side argument block
+    (usdu_stream_args) that `set` rewrites before every replay, so one captured graph serves every caller's tensors."""
+
+    def __init__(self, canvas: Canvas, order: Sequence[int], n_bands: int, max_ctas: int):
+        self.q, self.d = canvas.plan.stream_bands(order, canvas.B, n_bands, canvas.path_crop, canvas.path_blend)
+        dev = canvas.buf.device
+        self.args = torch.zeros(nat.STREAM_ARGS_BYTES, dtype=torch.uint8, device=dev)
+        self.stream = torch.cuda.Stream(device=dev)
+        self.max_ctas = max_ctas
+        self.full = max(nat.sm_count(), 1) * 128
+        self._ev: List[torch.cuda.Event] = []
+        self._waited: Dict[int, int] = {}
+
+    @staticmethod
+    def eligible(canvas: Canvas) -> bool:
+        return canvas.plan.W % 4 == 0
+
+    def set(self, image: torch.Tensor, out: torch.Tensor):
+        nat.stream_args_set(self.args.data_ptr(), image.data_ptr(), out.data_ptr(), _stream_ptr())
+
+    def start(self, canvas: Canvas, main: "torch.cuda.Stream"):
+        """Fork the streaming stream off `main` and enqueue every quantise band on it."""
+        p, s = canvas.plan, self.stream
+        self._ev, self._waited = [], {}
+        fork = torch.cuda.Event()
+        fork.record(main)
+        s.wait_event(fork)
+        with torch.cuda.stream(s):
+            for i, (y0, y1, _) in enumerate(self.q):
+                nat.quantize_rows_streamed(self.args.data_ptr(), canvas.buf.data_ptr(), canvas.B, p.H, p.W, canvas.pitch, y0, y1,
+                                           self.full if i == 0 else self.max_ctas, _stream_ptr())
+                canvas.launches += 1
+                e = torch.cuda.Event()
+                e.record(s)
+                self._ev.append(e)
+
+    def need(self, k: int, stream: "torch.cuda.Stream"):
+        """`stream` waits for every quantise band that wave k touches (the bands run in order: the last one suffices)."""
+        j = max((i for i, b in enumerate(self.q) if b[2] <= k), default=-1)
+        if j > self._waited.get(id(stream), -1):
+            stream.wait_event(self._ev[j])
+            self._waited[id(stream)] = j
+
+    def after_blend(self, k: int, canvas: Canvas, main: "torch.cuda.Stream"):
+        """Fork the dequantise bands whose rows no wave after k writes."""
+        bands = [i for i, b in enumerate(self.d) if b[2] == k]
+        if not bands:
+            return
+        p, s = canvas.plan, self.stream
+        e = torch.cuda.Event()
+        e.record(main)
+        s.wait_event(e)
+        with torch.cuda.stream(s):
+            for i in bands:
+                y0, y1, _ = self.d[i]
+                nat.dequantize_rows_streamed(canvas.buf.data_ptr(), self.args.data_ptr(), canvas.B, p.H, p.W, canvas.pitch, y0, y1,
+                                             self.full if i == len(self.d) - 1 else self.max_ctas, _stream_ptr())
+                canvas.launches += 1
+
+    def join(self, main: "torch.cuda.Stream"):
+        e = torch.cuda.Event()
+        e.record(self.stream)
+        main.wait_event(e)
+
+
 def use_split(canvas: Canvas, order: Sequence[int]) -> bool:
     """USDU_SCHEDULE=split*: level waves whose crop (and blend) launches are split by what the NEXT level really needs."""
     return SCHEDULE.startswith("split") and not FUSE_LEVELS and canvas.path_crop >= 1 and canvas.path_blend >= 1 and len(canvas.plan.waves(order)) > 2
 
 
 def run_split(canvas: Canvas, order: Sequence[int], denoiser: Denoiser, s_rest: "torch.cuda.Stream",
-              s_early: "torch.cuda.Stream", skip: Sequence[str] = ()) -> bool:
+              s_early: "torch.cuda.Stream", skip: Sequence[str] = (), casts: Optional[CastBands] = None) -> bool:
     """run_progressive(order) with every level's two launches split by dependency (planner.split_level); meant to be
     stream-captured.  single_gpu.py:40-64 orders a crop only after the blends that CHANGE pixels it reads:
       * crop(k+1) = `late` jobs (their staged rectangle meets a feather support of wave k) + `early` jobs, which run on
@@ -541,7 +621,9 @@ def run_split(canvas: Canvas, order: Sequence[int], denoiser: Denoiser, s_rest: 
     that run side by side never write the same block, and a crop beside a blend only ever reads bytes whose value the
     blend leaves as it is.  False (nothing launched) when a wave has no job-record lists.
     SCHEDULE: "split_crop" (default) splits only the crops; "split_blend" and "split" (both) also split the blends,
-    whose join takes the programmatic edge away from the critical blend.  skip: bench.py's differencing measurement -- the same schedule minus one kernel kind."""
+    whose join takes the programmatic edge away from the critical blend.  skip: bench.py's differencing measurement -- the same schedule minus one kernel kind.
+    casts: the canvas quantise / dequantise bands (CastBands, split_crop only) run inside the same graph: a crop waits
+    for the quantise bands it reads, a dequantise band forks after the last blend that writes its rows."""
     plan, B = canvas.plan, canvas.B
     waves = [_sorted_by_shape(plan, w) for w in plan.waves(order)]
     lists = canvas.dp.split_lists(waves, B, canvas.path_crop, canvas.path_blend)
@@ -570,6 +652,10 @@ def run_split(canvas: Canvas, order: Sequence[int], denoiser: Denoiser, s_rest: 
     keep = []                                     # tensors another stream still reads: released at the joins
     new_buf = torch.zeros if no_crop else torch.empty
     bufs[0] = new_buf(lists[0]["total"], dtype=torch.float32, device=dev)
+    if casts is not None:
+        if SCHEDULE != "split_crop" or skip:
+            raise ValueError("canvas cast bands run only with the split_crop schedule")
+        casts.start(canvas, main)
 
     def fork_early(k):                            # the crop jobs of wave k+1 that do not read what wave k changes
         if k + 1 < len(waves):
@@ -577,6 +663,8 @@ def run_split(canvas: Canvas, order: Sequence[int], denoiser: Denoiser, s_rest: 
             bufs[k + 1] = new_buf(N["total"], dtype=torch.float32, device=dev)
             if N["early"] is not None:
                 s_early.wait_event(event(main))
+                if casts is not None:
+                    casts.need(k + 1, s_early)
                 with torch.cuda.stream(s_early):
                     canvas.crop_jobs(N["early"][0], N["early"][1], bufs[k + 1])
                     early_done[k + 1] = event(s_early)
@@ -586,6 +674,8 @@ def run_split(canvas: Canvas, order: Sequence[int], denoiser: Denoiser, s_rest: 
         if fork_at == 0:
             fork_early(k)
         buf, offs = bufs[k], L["offs"]
+        if casts is not None:
+            casts.need(k, main)
         if L["late"] is not None and early_done[k] is not None:
             canvas.crop_jobs(L["late"][0], L["late"][1], buf)
             if fork_at == 1:
@@ -614,9 +704,13 @@ def run_split(canvas: Canvas, order: Sequence[int], denoiser: Denoiser, s_rest: 
             fork_early(k)
         if not no_blend:
             canvas.blend_jobs(L["crit"][0], L["crit"][1], None, out)
+        if casts is not None:
+            casts.after_blend(k, canvas, main)
         bufs[k] = None
     if rest_done is not None:
         main.wait_event(rest_done)
+    if casts is not None:
+        casts.join(main)
     # (every launch on the side streams is already joined through its event; a stream that never joined the capture must
     # not be waited for)
     return True
@@ -633,7 +727,9 @@ class GraphedWaves:
     def __init__(self, dp: DevicePlan, B: int, denoiser: Denoiser, profile: Optional[KernelProfile],
                  order: Optional[Sequence[int]] = None, keep_processed: bool = False,
                  payload: Optional[torch.Tensor] = None, where: Optional[dict] = None, skip: Sequence[str] = (),
-                 canvas_buf: Optional[torch.Tensor] = None, external_crop: bool = False):
+                 canvas_buf: Optional[torch.Tensor] = None, external_crop: bool = False, casts: bool = False):
+        """casts: the graph also quantises the caller's image and dequantises the result (CastBands; replay_job) when
+        the split_crop schedule runs; otherwise the caller fills the canvas and reads it back around the replay."""
         global PROFILE
         self.canvas = Canvas(dp, B, canvas_buf)
         self.denoiser = denoiser
@@ -662,23 +758,31 @@ class GraphedWaves:
                       and use_split(self.canvas, order))
         if self.split:
             lanes = [torch.cuda.Stream(device=dp.device), torch.cuda.Stream(device=dp.device)]
+        self.casts = None
+        if (casts and STREAM_OVERLAP and self.split and SCHEDULE == "split_crop" and not skip and canvas_buf is None
+                and CastBands.eligible(self.canvas)):
+            self.casts = CastBands(self.canvas, order, STREAM_BANDS, STREAM_CTAS)
 
-        def body():
+        def body(warm_up=False):
             if self.dag:
                 run_dag(self.canvas, order, denoiser, lanes, self.payload, where, skip)
                 return {}
-            if self.split and run_split(self.canvas, order, denoiser, lanes[0], lanes[1], skip):
+            if self.split and run_split(self.canvas, order, denoiser, lanes[0], lanes[1], skip, None if warm_up else self.casts):
                 return {}
+            if self.casts is not None:
+                raise nat.NativeError("canvas cast bands need the split schedule's job-record work lists")
             return run_progressive(self.canvas, order, denoiser, keep_processed, self.payload, where, skip, self.crop_buf)
 
-        with torch.cuda.stream(side):                 # warm-up: fills every cache (work lists, noise)
-            body()
+        with torch.cuda.stream(side):                 # warm-up: fills every cache (work lists, noise); no casts (no image yet)
+            body(warm_up=True)
         torch.cuda.current_stream(dp.device).wait_stream(side)
         torch.cuda.synchronize(dp.device)
         self.canvas.launches = 0
         self.canvas.algo_bytes = 0
         PROFILE = profile
-        self.graph = torch.cuda.CUDAGraph()
+        # with the cast bands the graph is instantiated here (usdu_graph_instantiate: node priorities), not by torch
+        self.graph = torch.cuda.CUDAGraph(keep_graph=self.casts is not None)
+        self.exec = None
         if profile is not None:
             profile.capturing = True
         try:
@@ -688,24 +792,52 @@ class GraphedWaves:
             PROFILE = saved
             if profile is not None:
                 profile.capturing = False
+        if self.casts is not None:
+            self.exec = nat.graph_instantiate(self.graph.raw_cuda_graph(), STREAM_PRIORITY)
         self.launches_per_replay = self.canvas.launches
         self.bytes_per_replay = self.canvas.algo_bytes
+
+    def __del__(self):
+        if getattr(self, "exec", None):
+            nat.graph_exec_destroy(self.exec)
+            self.exec = None
 
     @classmethod
     def get(cls, dp: DevicePlan, B: int, denoiser: Denoiser, profile: Optional[KernelProfile] = None,
             order: Optional[Sequence[int]] = None, keep_processed: bool = False,
             payload: Optional[torch.Tensor] = None, where: Optional[dict] = None, skip: Sequence[str] = (),
-            canvas_buf: Optional[torch.Tensor] = None, external_crop: bool = False) -> "GraphedWaves":
+            canvas_buf: Optional[torch.Tensor] = None, external_crop: bool = False, casts: bool = False) -> "GraphedWaves":
         pkey = None if payload is None else (payload.data_ptr(), payload.numel())
         ckey = None if canvas_buf is None else canvas_buf.data_ptr()
+        ckey_casts = (STREAM_OVERLAP, STREAM_CTAS, STREAM_BANDS, STREAM_PRIORITY) if casts else None
         key = (id(dp), B, getattr(denoiser, "graph_key", id(denoiser)), id(profile), FORCE_GENERIC, FORCE_NO_MMA, SCHEDULE, FUSE_LEVELS,
-               None if order is None else tuple(order), keep_processed, pkey, tuple(skip), ckey, external_crop)
+               None if order is None else tuple(order), keep_processed, pkey, tuple(skip), ckey, external_crop, ckey_casts)
         return cls._cache.get_or_build(
             key, lambda: GraphedWaves(dp, B, denoiser, profile, order, keep_processed, payload, where, skip, canvas_buf,
-                                      external_crop), lambda gw: gw.canvas.dp is dp)
+                                      external_crop, casts), lambda gw: gw.canvas.dp is dp)
+
+    def replay_job(self, image: torch.Tensor) -> torch.Tensor:
+        """The whole job on the caller's fp32 image -> a new fp32 result: with cast bands one replay of the graph, which
+        quantises, runs the wave loop and dequantises; otherwise Q0 (eager), the captured wave loop, the dequantise."""
+        if self.casts is None:
+            return self.replay(image).result()
+        c, p = self.canvas, self.canvas.plan
+        _require_cuda(image, "image")
+        if tuple(image.shape) != (c.B, p.H, p.W, 3) or image.dtype != torch.float32:
+            raise ValueError(f"image must be float32 [{c.B},{p.H},{p.W},3], got {image.dtype} {tuple(image.shape)}")
+        image = image.contiguous()
+        if image.data_ptr() % 16:                  # the vector loads of the streamed quantise
+            image = image.clone()
+        out = torch.empty((c.B, p.H, p.W, 3), dtype=torch.float32, device=c.buf.device)
+        c.launches, c.algo_bytes = self.launches_per_replay, self.bytes_per_replay
+        self.casts.set(image, out)
+        nat.graph_launch(self.exec, _stream_ptr())
+        return out
 
     def replay(self, image: torch.Tensor) -> Canvas:
         """Q0 from the caller's tensor (eager), then the captured wave loop."""
+        if self.casts is not None:
+            raise ValueError("this graph quantises its input itself: use replay_job")
         c = self.canvas
         c.launches, c.algo_bytes = self.launches_per_replay, self.bytes_per_replay
         c.load(image)
@@ -742,11 +874,13 @@ def upscale_single(image: torch.Tensor, denoiser: Denoiser, tile_width: int, til
     with torch.cuda.device(image.device):
         dp = DevicePlan.get(plan, image.device)
         if use_graph:
-            canvas = GraphedWaves.get(dp, B, denoiser, PROFILE, skip=_skip).replay(image)
+            gw = GraphedWaves.get(dp, B, denoiser, PROFILE, skip=_skip, casts=True)
+            res = gw.replay_job(image)
+            canvas = gw.canvas
         else:
             canvas = Canvas(dp, B).load(image)
             run_progressive(canvas, range(len(plan.tiles)), denoiser)
-        res = canvas.result()
+            res = canvas.result()
     if stats is not None:
         stats["gpu_launches"] = stats.get("gpu_launches", 0) + canvas.launches
         stats["algo_bytes"] = stats.get("algo_bytes", 0) + canvas.algo_bytes

@@ -344,6 +344,58 @@ class Plan:
         rest = self.blend_worklist(wave, offs, 4, path, B, blocks=(rects, False))
         return cr, coffs, ctotal, late, crit, rest
 
+    CROP_BOX_ROWS = (0, 40, 48)           # rows of a crop's bulk-tensor box per kernel path (usdu_fast.cu / usdu_mma.cu kBoxR)
+
+    def wave_rows(self, waves: Sequence[Sequence[int]], B: int, path_crop: int = 2, path_blend: int = 2):
+        """Per dependency wave, the canvas rows its launches can touch (job records of the crop and blend work lists,
+        path >= 1): -> (touch, write), bool [len(waves), H].  touch = rows a crop's TMA box can load (the whole box from its
+        first staged row, plus the next row for the integer-pipe staging's 16-byte over-read) or a blend block loads;
+        write = rows of whole blend blocks, which a blend stores back even where the mask leaves them unchanged."""
+        touch = np.zeros((len(waves), self.H), dtype=bool)
+        write = np.zeros((len(waves), self.H), dtype=bool)
+        for k, wave in enumerate(waves):
+            cr, offs, _ = self.crop_worklist(wave, B, path_crop)
+            bl = self.blend_worklist(wave, offs, 4, path_blend, B)
+            if cr.path < 1 or bl.path < 1:
+                raise ValueError("wave_rows needs job-record work lists (path >= 1)")
+            J = cr.items.reshape(-1, nat.JOB_WORDS)
+            box, slack = self.CROP_BOX_ROWS[cr.path], int(cr.path == 1)
+            for y0, n in zip(J[:, nat.J_SRC_B].tolist(), J[:, nat.J_ROWS].tolist()):
+                touch[k, max(y0, 0):min(y0 + max(n, box) + slack, self.H)] = True
+            J = bl.items.reshape(-1, nat.JOB_WORDS)
+            for y0, n in zip(J[:, nat.J_DST_Y].tolist(), J[:, nat.J_ROWS_OUT].tolist()):
+                write[k, max(y0, 0):min(y0 + max(n, bl.block_rows), self.H)] = True
+            touch[k] |= write[k]
+        return touch, write
+
+    def stream_bands(self, order: Optional[Sequence[int]], B: int, n_bands: int, path_crop: int = 2, path_blend: int = 2):
+        """Row bands of the canvas quantise and dequantise passes when they run beside the level waves of `order`
+        (engine.run_split).  -> (quantise, dequantise), lists of (y0, y1, wave): each quantise band [y0, y1) is tagged
+        with the FIRST wave that touches one of its rows (it must be complete before that wave's crops start), each
+        dequantise band with the LAST wave that writes one of its rows (it may start once that wave's blend is done).
+        Rows are those of every frame; each list covers [0, H) once, top to bottom.  The first quantise band is exactly
+        the rows the first wave touches (from row 0) and the last dequantise band the rows from the last wave's first
+        written row down; the rest of each pass is cut into n_bands - 1 bands of equal height."""
+        waves = self.waves(order)
+        touch, write = self.wave_rows(waves, B, path_crop, path_blend)
+        H, n_bands = self.H, max(1, int(n_bands))
+        lo = np.arange(len(waves))[:, None]
+        first = np.where(touch, lo, len(waves)).min(0)          # per row: first wave touching it
+        last = np.where(write, lo, -1).max(0)                    # per row: last wave writing it
+        if (last < 0).any():
+            raise ValueError("stream_bands: some canvas row is written by no wave")
+
+        def cut(y0, y1, n):
+            n = max(1, min(n, y1 - y0))
+            return [(y0 + (y1 - y0) * i // n, y0 + (y1 - y0) * (i + 1) // n) for i in range(n)]
+
+        q_head = int(np.nonzero(touch[0])[0].max()) + 1
+        q = [(0, q_head)] + (cut(q_head, H, n_bands - 1) if q_head < H and n_bands > 1 else [(q_head, H)] if q_head < H else [])
+        d_tail = int(np.nonzero(write[-1])[0].min())
+        d = (cut(0, d_tail, n_bands - 1) if d_tail > 0 and n_bands > 1 else [(0, d_tail)] if d_tail > 0 else []) + [(d_tail, H)]
+        return ([(y0, y1, int(first[y0:y1].min())) for y0, y1 in q],
+                [(y0, y1, int(last[y0:y1].max())) for y0, y1 in d])
+
     MAX_LEVEL_DEPS = 4
 
     def level_worklist(self, blend_ids: Sequence[int], offs: np.ndarray, crop_ids: Sequence[int], B: int, share: int = 1):

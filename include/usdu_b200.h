@@ -35,7 +35,7 @@ extern "C" {
 #pragma GCC visibility push(default) /* the library itself is built with -fvisibility=hidden */
 #endif
 
-#define USDU_ABI_VERSION 9
+#define USDU_ABI_VERSION 10
 
 typedef enum usdu_status {
     USDU_OK = 0,
@@ -242,6 +242,29 @@ int usdu_quantize_rows(const float* img_dev, uint8_t* canvas_dev, int B, int H, 
                        int y0, int y1, void* stream);
 int usdu_dequantize_rows(const uint8_t* canvas_dev, float* img_dev, int B, int H, int W, int64_t pitch,
                          int y0, int y1, void* stream);
+/* The same two casts as launches a captured CUDA graph can replay for any caller's tensors, meant to run in row bands
+ * on a side stream beside the wave loop.  The fp32 image (quantise) and result (dequantise) are not launch arguments:
+ * each kernel reads them from a DEVICE-resident usdu_stream_args block, which usdu_stream_args_set rewrites on `stream`
+ * before the graph is replayed there (one 16-byte copy; the host array is staged by the driver before the call returns,
+ * so back-to-back calls need no pinned buffer).  At most max_ctas CTAs stride over the band (1 <= max_ctas): a
+ * bandwidth-bound pass that holds only a few CTA slots leaves the others to the latency-bound wave kernels.  Needs W % 4
+ * == 0 and 16-byte aligned canvas, image and result (checked here and by usdu_stream_args_set). */
+typedef struct usdu_stream_args {
+    const float* img_dev;   /* [B][H][W][3] input of usdu_quantize_rows_streamed */
+    float* out_dev;         /* [B][H][W][3] result of usdu_dequantize_rows_streamed */
+} usdu_stream_args;
+int usdu_stream_args_set(usdu_stream_args* args_dev, const float* img_dev, float* out_dev, void* stream);
+int usdu_quantize_rows_streamed(const usdu_stream_args* args_dev, uint8_t* canvas_dev, int B, int H, int W, int64_t pitch,
+                                int y0, int y1, int max_ctas, void* stream);
+int usdu_dequantize_rows_streamed(const uint8_t* canvas_dev, const usdu_stream_args* args_dev, int B, int H, int W,
+                                  int64_t pitch, int y0, int y1, int max_ctas, void* stream);
+/* Instantiate a captured graph (cudaGraph_t passed as void*) for replay.  high_priority != 0: every kernel node except
+ * the two streamed casts above gets the device's greatest stream priority and the graph is instantiated with
+ * cudaGraphInstantiateFlagUseNodePriority, so the wave kernels win CTA dispatch over a cast band running beside them.
+ * *exec_out receives the cudaGraphExec_t; launch it with usdu_graph_launch, free it with usdu_graph_exec_destroy. */
+int usdu_graph_instantiate(void* graph, int high_priority, void** exec_out);
+int usdu_graph_launch(void* exec, void* stream);
+int usdu_graph_exec_destroy(void* exec);
 /* The master's gather of a multi-GPU job in ONE launch: canvas rows [slab_rows[q], slab_rows[q+1]) are read from
  * slab_canvas_dev[q] (host array of n_slabs device pointers, each the base of a whole [B][H][pitch] canvas: the local one
  * or a peer's mapped over NVLink) and dequantised into the local fp32 image.  slab_rows (host, n_slabs + 1 ints) must
