@@ -889,6 +889,47 @@ def upscale_single(image: torch.Tensor, denoiser: Denoiser, tile_width: int, til
     return res
 
 
+class WorkerJob:
+    """The device state of one static-mode worker of the reference's HTTP master for one job (static.py:191-314): the
+    worker's own u8 canvas in HBM, and per tile id the master hands out a 1-tile step -- crop from this canvas, sampler,
+    truncating u8 pack of the sampler output, blend into this canvas.  Each crop sees this worker's earlier blends and
+    nothing else, as in static.py:242-280.  The packed tile is what the reference's worker PNG-encodes
+    (`tensor_to_pil(processed_batch, b)`, worker_comms.py:30): the sampler output at processing size."""
+
+    def __init__(self, image: torch.Tensor, denoiser: Denoiser, tile_width: int, tile_height: int, padding: int,
+                 mask_blur: int, force_uniform_tiles: bool = True, device: Optional[torch.device] = None):
+        self.device = image.device if image.is_cuda else (device or torch.device("cuda", torch.cuda.current_device()))
+        x = reference_f32(image).contiguous()
+        B, H, W, _ = x.shape
+        self.plan = get_plan(W, H, tile_width, tile_height, padding, mask_blur, force_uniform_tiles)
+        self.denoiser = denoiser
+        self.times = {"device_ms": 0.0, "d2h_ms": 0.0, "tiles": 0}    # CUDA-event totals over step()
+        with torch.cuda.device(self.device):
+            if not x.is_cuda:                    # uploaded once; the canvas is all the job keeps
+                x = (x if x.is_pinned() else x.pin_memory()).to(self.device, non_blocking=True)
+            self.canvas = Canvas(DevicePlan.get(self.plan, self.device), B).load(x)
+            torch.cuda.current_stream().synchronize()     # the fp32 upload may be freed now
+
+    def step(self, tile_id: int) -> np.ndarray:
+        """Process tile `tile_id` -> its u8 payload [B, ph, pw, 3] in page-locked host memory."""
+        tile_id = int(tile_id)
+        if not 0 <= tile_id < len(self.plan.tiles):
+            raise ValueError(f"tile id {tile_id} is outside this job's {len(self.plan.tiles)} tiles")
+        with torch.cuda.device(self.device):
+            e0, e1, e2 = (torch.cuda.Event(enable_timing=True) for _ in range(3))
+            e0.record()
+            q = run_progressive(self.canvas, [tile_id], self.denoiser, keep_processed=True)[tile_id]
+            e1.record()
+            host = torch.empty(q.shape, dtype=torch.uint8, pin_memory=True)
+            host.copy_(q, non_blocking=True)
+            e2.record()
+            e2.synchronize()
+        self.times["device_ms"] += e0.elapsed_time(e1)
+        self.times["d2h_ms"] += e1.elapsed_time(e2)
+        self.times["tiles"] += 1
+        return host.numpy()
+
+
 # --------------------------------------------------------------------------------------
 # host-tensor path: H2D, compute and D2H overlapped band by band
 # --------------------------------------------------------------------------------------

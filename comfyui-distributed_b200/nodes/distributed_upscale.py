@@ -2,13 +2,16 @@
 nodes/distributed_upscale.py:46-279, running the tile path on the H100 kernels.
 
 What changes behind the signature:
-* pixels never touch PIL or the CPU: the canvas lives in HBM as u8, crop / feather /
-  blend are sm_90a kernels (engine.py);
+* pixels never touch PIL or the CPU (except the PNG tiles an HTTP worker posts, below): the canvas lives in HBM as u8,
+  crop / feather / blend are sm_90a kernels (engine.py);
 * "workers" are torch.distributed ranks (one process per GPU, NCCL); the hidden inputs
   injected by the reference's orchestrator (multi_job_id, is_worker, master_url,
   enabled_worker_ids, worker_id, tile_indices, dynamic_threshold) are accepted and
   validated the same way, but the role comes from the rank (rank 0 = master);
 * the tile pull-queue becomes a static plan (planner.partition);
+* started by the reference's orchestrator as a worker (no torch.distributed peers), the node is a static-mode worker of
+  the reference's HTTP master: tiles are pulled and posted back as PNGs (http_worker.py), each computed on this GPU
+  against the worker's own u8 canvas (engine.WorkerJob);
 * `semantics` (class / instance attribute, default from USDU_SEMANTICS, not a widget -- the signature stays the
   reference's): "static" = the reference's multi-worker result for that plan (upscale/modes/static.py); "exact" = the
   N ranks cooperatively compute the reference's SINGLE-GPU result (single_gpu.py:8-72), bit-identical at any world size
@@ -24,7 +27,8 @@ import torch
 from .. import dist as usdu_dist
 from ..casts import reference_f32
 from ..denoise import ComfySampler
-from ..engine import upscale_host, upscale_single
+from ..engine import WorkerJob, upscale_host, upscale_single
+from ..http_worker import HttpStaticWorker
 
 try:  # ComfyUI supplies these lists; outside ComfyUI keep the signature importable
     import comfy.samplers as _cs
@@ -115,13 +119,18 @@ class UltimateSDUpscaleDistributed:
         dev = src_device if upscaled_image.is_cuda else torch.device("cuda", torch.cuda.current_device())
         self.last_stats = {"time_phases": True} if getattr(self, "time_phases", False) else {}
         if multi_job_id and is_worker and world == 1:
-            # The reference's HTTP orchestrator started this process as a worker (static.py:191-314).  Its tile queue
-            # and PNG transport are not part of this package (an SPMD launch, one rank per GPU, replaces them): do what
-            # a worker does for the graph -- hand the input through (static.py:314) -- and say why no tile was processed.
-            import warnings
-            warnings.warn("UltimateSDUpscaleDistributed (CUDA tile path): running as an HTTP worker of the reference's orchestrator is "
-                          "not supported; launch one rank per GPU with torch.distributed instead. Returning the input.",
-                          RuntimeWarning, stacklevel=2)
+            # The reference's HTTP orchestrator started this process as a worker (static.py:191-314): pull tile ids from
+            # its master, process each on this GPU against this worker's own canvas, post the PNG tiles back, and hand
+            # the input through (static.py:314).
+            _, H, W, _ = upscaled_image.shape
+            denoiser = self._make_denoiser(model, positive, negative, vae, seed, steps, cfg, sampler_name, scheduler,
+                                           denoise, tiled_decode, (W, H))
+            job = WorkerJob(upscaled_image, denoiser, tile_width, tile_height, padding, mask_blur, force_uniform_tiles,
+                            device=dev)
+            worker = HttpStaticWorker(master_url, multi_job_id, worker_id, padding,
+                                      [(t.x1, t.y1, t.ew, t.eh) for t in job.plan.tiles], job.canvas.B)
+            worker.run(job.step)
+            self.last_stats.update(pulled=list(worker.pulled), chunks=worker.chunks)
             return (upscaled_image,)
         if self.semantics not in ("static", "exact"):
             raise ValueError(f"semantics must be 'static' or 'exact', got {self.semantics!r}")
