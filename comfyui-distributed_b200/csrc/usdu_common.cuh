@@ -35,6 +35,18 @@ inline int grid_sms() { const int n = sm_count(); return n > 0 ? n : 1; }
         if (_s != USDU_OK) return _s;                                \
     } while (0)
 
+// Let kernel `fn` launch with `bytes` of dynamic shared memory on the current device: raise its limit, never lower it.
+// A launch captured into a CUDA graph keeps its size after later, smaller launches of the same kernel; a limit lowered
+// below it makes the runtime reject that node (cudaGraphKernelNodeSetAttribute, instantiation: "invalid argument").
+inline int raise_smem_limit(const void* fn, size_t bytes) {
+    if (bytes <= 48 * 1024) return USDU_OK;
+    cudaFuncAttributes a;
+    USDU_CUDA(cudaFuncGetAttributes(&a, fn));
+    if ((size_t)a.maxDynamicSharedSizeBytes < bytes)
+        USDU_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+    return USDU_OK;
+}
+
 // (uint8)(255.f * x): fp32 multiply (round to nearest), C truncation, wrap to 8 bits.
 // utils/image.py:8-10 -- numpy's float32 -> uint8 cast on x86: cvttss2si, then the low byte.  cvttss2si returns
 // 0x80000000 for NaN, +-inf and every product outside [-2^31, 2^31), so all of those give 0.  cvt.rzi.s32 gives 0

@@ -421,8 +421,7 @@ static int optin(const void* fn, size_t bytes) {
         set_error("fast kernel needs %zu bytes of shared memory (> 227 KB)", bytes);
         return USDU_ERR_UNSUPPORTED;
     }
-    if (bytes > 48 * 1024) USDU_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-    return USDU_OK;
+    return raise_smem_limit(fn, bytes);
 }
 
 int launch_crop(const uint8_t* canvas, int B, int H, int W, int64_t pitch, const int32_t* tiles, const int32_t* tabs,

@@ -246,15 +246,21 @@ __device__ __forceinline__ void axis_range(const int32_t* tabs, int tab, int o0,
     }
 }
 
-// Horizontal pass: in[rows][in_pitch] (u8, pixel-interleaved, column 0 == input pixel ix0)
-// -> mid[rows][mid_pitch] holding `ow` output pixels starting at output index ox0.
-__device__ __forceinline__ void hpass(const uint8_t* in, int in_pitch, int ix0, uint8_t* mid, int mid_pitch,
+// A source byte of the horizontal pass: u8 as it is, fp32 through the truncating cast Q1.
+__device__ __forceinline__ uint32_t load8(const uint8_t* p) { return *p; }
+__device__ __forceinline__ uint32_t load8(const float* p) { return quant_u8(__ldg(p)); }
+
+// Horizontal pass: in[rows][in_pitch] (u8 or fp32, pixel-interleaved, column 0 == input pixel ix0; the patch staged in
+// shared memory, or the source itself in global memory) -> mid[rows][mid_pitch] holding `ow` output pixels starting at
+// output index ox0.
+template <typename T>
+__device__ __forceinline__ void hpass(const T* in, int64_t in_pitch, int ix0, uint8_t* mid, int mid_pitch,
                                       int rows, int ox0, int ow, const int32_t* tabs, int tab) {
     const int ow3 = ow * 3;
     if (tab < 0) {
         for (int i = threadIdx.x; i < rows * ow3; i += blockDim.x) {
             const int r = i / ow3, j = i - r * ow3;
-            mid[r * mid_pitch + j] = in[r * in_pitch + j];
+            mid[r * mid_pitch + j] = (uint8_t)load8(in + r * in_pitch + j);
         }
         return;
     }
@@ -264,13 +270,13 @@ __device__ __forceinline__ void hpass(const uint8_t* in, int in_pitch, int ix0, 
         const int xmin = __ldg(t.bounds + 2 * (ox0 + xx));
         const int n = __ldg(t.bounds + 2 * (ox0 + xx) + 1);
         const int32_t* k = t.kk + (int64_t)(ox0 + xx) * t.ksize;
-        const uint8_t* p = in + r * in_pitch + (xmin - ix0) * 3;
+        const T* p = in + r * in_pitch + (xmin - ix0) * 3;
         int a0 = 1 << (kPrecisionBits - 1), a1 = a0, a2 = a0;
         for (int q = 0; q < n; ++q) {
             const int kv = __ldg(k + q);
-            a0 += p[3 * q] * kv;
-            a1 += p[3 * q + 1] * kv;
-            a2 += p[3 * q + 2] * kv;
+            a0 += (int)load8(p + 3 * q) * kv;
+            a1 += (int)load8(p + 3 * q + 1) * kv;
+            a2 += (int)load8(p + 3 * q + 2) * kv;
         }
         uint8_t* o = mid + r * mid_pitch + xx * 3;
         o[0] = (uint8_t)clip8(a0 >> kPrecisionBits);
@@ -344,7 +350,10 @@ crop_resize_kernel(const uint8_t* __restrict__ canvas, int H, int W, int64_t pit
 // ======================================================================================
 // K4: quantise + LANCZOS back + integer alpha composite, per canvas block
 // ======================================================================================
-template <bool kSrcU8>
+// kDirect: the patch of the processed tile a block reads would not fit in shared memory (a canvas far smaller than the
+// tile: 2304 -> 64 px back-resizes 324 x 324 pixels into a 4 x 4 block); the horizontal pass then reads (and quantises)
+// the tile in global memory and only the intermediate [max_rows][blk_w*3] is staged.
+template <bool kSrcU8, bool kDirect>
 __global__ void __launch_bounds__(kThreads)
 blend_kernel(uint8_t* __restrict__ canvas, int H, int W, int64_t pitch, const int32_t* __restrict__ tiles,
              const int32_t* __restrict__ tabs, const uint8_t* __restrict__ mask_pool,
@@ -356,9 +365,10 @@ blend_kernel(uint8_t* __restrict__ canvas, int H, int W, int64_t pitch, const in
     const int bx0 = it[0], by0 = it[1];
     const int bw = min(blk_w, W - bx0), bh = min(blk_h, H - by0);
     const int d_pitch = BW * 3;
-    uint8_t* D = smem;                              // [BH][BW*3] canvas block
-    uint8_t* mid = D + BH * d_pitch;                // [max_rows][BW*3]
-    uint8_t* in = mid + (size_t)max_rows * d_pitch; // [max_rows][in_pitch]
+    const int mid_pitch = blk_w * 3;
+    uint8_t* D = smem;                                // [BH][BW*3] canvas block
+    uint8_t* mid = D + BH * d_pitch;                  // [max_rows][blk_w*3]
+    uint8_t* in = mid + (size_t)max_rows * mid_pitch; // [max_rows][in_pitch] (staged path)
 
     uint8_t* cblk = canvas + ((int64_t)b * H + by0) * pitch + (int64_t)bx0 * 3;
     const int bw3 = bw * 3;
@@ -384,25 +394,31 @@ blend_kernel(uint8_t* __restrict__ canvas, int H, int W, int64_t pitch, const in
         axis_range(tabs, tabV, oy0, oh, iy0, iy1);
         const int rows = iy1 - iy0, cols3 = (ix1 - ix0) * 3;
         __syncthreads();  // previous tile's composite (and the D load) done before in/mid are reused
-        // stage the processed-tile patch, quantised to u8 (Q1)
         const int64_t frame = (int64_t)ph * pw * 3;
-        if (kSrcU8) {
-            const uint8_t* s = static_cast<const uint8_t*>(src_v) + src_off + b * frame +
-                               ((int64_t)iy0 * pw + ix0) * 3;
-            for (int i = threadIdx.x; i < rows * cols3; i += blockDim.x) {
-                const int r = i / cols3, j = i - r * cols3;
-                in[r * in_pitch + j] = s[(int64_t)r * pw * 3 + j];
-            }
+        const int64_t s_off = src_off + b * frame + ((int64_t)iy0 * pw + ix0) * 3;
+        if (kDirect) {
+            if (kSrcU8)
+                hpass(static_cast<const uint8_t*>(src_v) + s_off, (int64_t)pw * 3, ix0, mid, mid_pitch, rows, ox0, ow, tabs, tabH);
+            else
+                hpass(static_cast<const float*>(src_v) + s_off, (int64_t)pw * 3, ix0, mid, mid_pitch, rows, ox0, ow, tabs, tabH);
         } else {
-            const float* s = static_cast<const float*>(src_v) + src_off + b * frame +
-                             ((int64_t)iy0 * pw + ix0) * 3;
-            for (int i = threadIdx.x; i < rows * cols3; i += blockDim.x) {
-                const int r = i / cols3, j = i - r * cols3;
-                in[r * in_pitch + j] = (uint8_t)quant_u8(__ldg(s + (int64_t)r * pw * 3 + j));
+            // stage the processed-tile patch, quantised to u8 (Q1)
+            if (kSrcU8) {
+                const uint8_t* s = static_cast<const uint8_t*>(src_v) + s_off;
+                for (int i = threadIdx.x; i < rows * cols3; i += blockDim.x) {
+                    const int r = i / cols3, j = i - r * cols3;
+                    in[r * in_pitch + j] = s[(int64_t)r * pw * 3 + j];
+                }
+            } else {
+                const float* s = static_cast<const float*>(src_v) + s_off;
+                for (int i = threadIdx.x; i < rows * cols3; i += blockDim.x) {
+                    const int r = i / cols3, j = i - r * cols3;
+                    in[r * in_pitch + j] = (uint8_t)quant_u8(__ldg(s + (int64_t)r * pw * 3 + j));
+                }
             }
+            __syncthreads();
+            hpass(in, in_pitch, ix0, mid, mid_pitch, rows, ox0, ow, tabs, tabH);
         }
-        __syncthreads();
-        hpass(in, in_pitch, ix0, mid, d_pitch, rows, ox0, ow, tabs, tabH);
         __syncthreads();
         const uint8_t* mk = mask_pool + (int64_t)(uint32_t)T[USDU_T_MASK_OFF] +
                             (int64_t)oy0 * T[USDU_T_MASK_PITCH] + ox0;
@@ -413,8 +429,8 @@ blend_kernel(uint8_t* __restrict__ canvas, int H, int W, int64_t pitch, const in
         if (tabV >= 0) tv = table_at(tabs, tabV);
         for (int i = threadIdx.x; i < oh * ow3; i += blockDim.x) {
             const int yy = i / ow3, j = i - yy * ow3;
-            const uint32_t S = (tabV < 0) ? mid[yy * d_pitch + j]
-                                          : vpass_at(mid, d_pitch, iy0, oy0 + yy, j, tv);
+            const uint32_t S = (tabV < 0) ? mid[yy * mid_pitch + j]
+                                          : vpass_at(mid, mid_pitch, iy0, oy0 + yy, j, tv);
             const uint32_t A = __ldg(mk + (int64_t)yy * mpitch + j / 3);
             uint8_t* d = Dw + yy * d_pitch + j;
             *d = (uint8_t)composite8(S, *d, A);
@@ -518,13 +534,14 @@ static inline int grid_for(int64_t blocks) {
     return (int)(blocks < 1 ? 1 : (blocks > cap ? cap : blocks));
 }
 
+constexpr size_t kMaxSmem = 227 * 1024;   // dynamic shared memory a CTA may opt in to on sm_90
+
 static int smem_optin(const void* fn, size_t bytes) {
-    if (bytes > 227 * 1024) {
+    if (bytes > kMaxSmem) {
         set_error("kernel needs %zu bytes of shared memory (> 227 KB): patch too large", bytes);
         return USDU_ERR_UNSUPPORTED;
     }
-    if (bytes > 48 * 1024) USDU_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-    return USDU_OK;
+    return raise_smem_limit(fn, bytes);
 }
 
 }  // namespace usdu
@@ -949,20 +966,21 @@ int usdu_tile_blend(uint8_t* canvas_dev, int B, int H, int W, int64_t pitch, con
                                   cover_dev, patch_w, patch_h, src_dev, src_is_u8, (flags >> 8) & 0xFF,
                                   (flags & USDU_FLAG_REMOTE_CANVAS) ? 1 : 0, (cudaStream_t)stream);
     }
-    const int in_pitch = (patch_w * 3 + 15) / 16 * 16;
-    const size_t smem = (size_t)BH * BW * 3 + (size_t)patch_h * BW * 3 + (size_t)patch_h * in_pitch;
-    const void* fn = src_is_u8 ? (const void*)blend_kernel<true> : (const void*)blend_kernel<false>;
-    int s = smem_optin(fn, smem);
-    if (s != USDU_OK) return s;
     int blk_h = (flags >> 8) & 0xFF, blk_w = (flags >> 16) & 0xFF;     // generic path: optional smaller blocks
     if (blk_h <= 0 || blk_h > BH) blk_h = BH;
     if (blk_w <= 0 || blk_w > BW) blk_w = BW;
-    if (src_is_u8)
-        blend_kernel<true><<<dim3(n_items, B), kThreads, smem, (cudaStream_t)stream>>>(
-            canvas_dev, H, W, pitch, tiles_dev, tabs_dev, mask_pool_dev, items_dev, cover_dev, src_dev, in_pitch, patch_h, blk_w, blk_h);
-    else
-        blend_kernel<false><<<dim3(n_items, B), kThreads, smem, (cudaStream_t)stream>>>(
-            canvas_dev, H, W, pitch, tiles_dev, tabs_dev, mask_pool_dev, items_dev, cover_dev, src_dev, in_pitch, patch_h, blk_w, blk_h);
+    const int in_pitch = (patch_w * 3 + 15) / 16 * 16;
+    const size_t head = (size_t)BH * BW * 3 + (size_t)patch_h * blk_w * 3;
+    const bool direct = head + (size_t)patch_h * in_pitch > kMaxSmem;  // the patch does not fit: read the tile itself
+    const size_t smem = direct ? head : head + (size_t)patch_h * in_pitch;
+    void (*fn)(uint8_t*, int, int, int64_t, const int32_t*, const int32_t*, const uint8_t*, const int32_t*, const int32_t*,
+               const void*, int, int, int, int) =
+        src_is_u8 ? (direct ? blend_kernel<true, true> : blend_kernel<true, false>)
+                  : (direct ? blend_kernel<false, true> : blend_kernel<false, false>);
+    int s = smem_optin((const void*)fn, smem);
+    if (s != USDU_OK) return s;
+    fn<<<dim3(n_items, B), kThreads, smem, (cudaStream_t)stream>>>(
+        canvas_dev, H, W, pitch, tiles_dev, tabs_dev, mask_pool_dev, items_dev, cover_dev, src_dev, in_pitch, patch_h, blk_w, blk_h);
     USDU_CUDA(cudaGetLastError());
     return USDU_OK;
 }

@@ -758,8 +758,7 @@ static int optin(const void* fn, size_t bytes) {
         set_error("tensor-core kernel needs %zu bytes of shared memory (> 227 KB)", bytes);
         return USDU_ERR_UNSUPPORTED;
     }
-    if (bytes > 48 * 1024) USDU_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-    return USDU_OK;
+    return raise_smem_limit(fn, bytes);
 }
 
 static int split_patch_h(int patch_h, int* plane_rows, int* mid_rows, const char* who) {

@@ -10,6 +10,8 @@ Outputs (committed, small):
   tests/golden/mask_crop.npz      crop_mask outputs (conditioning masks cut to a tile), u8
   tests/golden/static_ref_index.json   the reference's multi-worker static mode run over HTTP here: the tile
                                   assignment each run ended up with + SHA-256 of the master's u8 result
+  tests/golden/sweep_ref_digests.json, wide_ref_digests.json   SHA-256 of process_single_gpu's u8 output for the
+                                  seeded parameter sweep and for the wide tile / padding / blur range cases
 
 Test infrastructure only (see oracle/usdu_oracle.py header).
 """
@@ -32,7 +34,8 @@ OUT = os.path.join(os.path.dirname(HERE), "tests", "golden")
 
 
 sys.path.insert(0, os.path.join(os.path.dirname(HERE), "tests"))
-from inputs import MASK_CROP_CASES, STATIC_REF_CASES, make_input, make_mask, sweep_cases, sweep_sampler  # noqa: E402  (shared with the tests)
+from inputs import (MASK_CROP_CASES, STATIC_REF_CASES, WIDE_CASES, make_input, make_mask, sweep_cases,  # noqa: E402  (shared with the tests)
+                    sweep_sampler, wide_sampler)
 
 
 def torch_t0(seed_unused=None):
@@ -144,10 +147,36 @@ def gen_sweep_digests():
         json.dump({"generator": "oracle/gen_golden.py", "reference": "a91f9fb", "digests": digests}, f, indent=1)
 
 
+def gen_wide_digests():
+    """tests/golden/wide_ref_digests.json: SHA-256 of the REAL reference's process_single_gpu output (u8) for the
+    whole-job cases of the wide-range tests (tests/inputs.py WIDE_CASES): tiles up to 2048, padding up to 256, blur up
+    to 256, canvases far smaller than a tile.  Each is also checked against the oracle's process_single here."""
+    node, fake_nodes = ref_loader.make_reference_node()
+    digests = {}
+    for (i, B, H, W, tw, th, pad, blur, uni, job) in WIDE_CASES:
+        if not job:
+            continue
+        seed, den = wide_sampler(i)
+        fake_nodes.fn = torch_t0()
+        img = make_input("noise", i, B, H, W)
+        (res,) = node.process_single_gpu(torch.from_numpy(img), None, [[torch.zeros(1, 77, 8), {}]],
+                                         [[torch.zeros(1, 77, 8), {}]], None, seed, 20, 8.0, "euler", "normal", den,
+                                         tw, th, pad, blur, uni, False)
+        out = np.round(res.numpy() * 255).astype(np.uint8)
+        assert np.array_equal(out.astype(np.float32) / np.float32(255), res.numpy())
+        assert np.array_equal(orc.process_single(img, orc.make_t0_denoiser(seed, den), tw, th, pad, blur, uni), res.numpy()), i
+        digests[str(i)] = hashlib.sha256(out.tobytes()).hexdigest()
+        print("wide", i, B, H, W, tw, th, pad, blur, uni, digests[str(i)][:16], flush=True)
+    with open(os.path.join(OUT, "wide_ref_digests.json"), "w") as f:
+        json.dump({"generator": "oracle/gen_golden.py", "reference": "a91f9fb", "digests": digests}, f, indent=1)
+
+
 def main():
     os.makedirs(OUT, exist_ok=True)
     if "--sweep-only" in sys.argv:
         return gen_sweep_digests()
+    if "--wide-only" in sys.argv:
+        return gen_wide_digests()
     if "--mask-crop-only" in sys.argv:
         return gen_mask_crop()
     if "--static-ref-only" in sys.argv:
@@ -155,6 +184,7 @@ def main():
     gen_mask_crop()
     gen_static_ref()
     gen_sweep_digests()
+    gen_wide_digests()
     node, fake_nodes = ref_loader.make_reference_node()
     fake_nodes.fn = torch_t0()
 

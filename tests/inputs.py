@@ -90,3 +90,31 @@ def sweep_cases():
 
 def sweep_sampler(i: int):
     return 1000 + i, 0.25 + 0.05 * (i % 10)
+
+
+# (id, B, H, W, tile_w, tile_h, padding, mask_blur, uniform, whole_job) -- the node's tile / padding / blur range up to its
+# limits (tests/test_gpu_wide_range.py).  whole_job: also run end to end; the real reference's digests of those jobs are in
+# tests/golden/wide_ref_digests.json (oracle/gen_golden.py gen_wide_digests; input "noise" seed = id, sampler wide_sampler).
+WIDE_CASES = [
+    (0, 1, 500, 700, 128, 128, 48, 8, True, True),          # tensor-core crop staged with LDG (patch > 48 rows)
+    (1, 1, 500, 700, 128, 128, 96, 8, True, True),          # ... with two k-steps (crop down-scale ~1.5)
+    (2, 2, 400, 520, 128, 128, 96, 8, True, True),          # ... also from the fp32 image; two-k-step blend, 16-row blocks
+    (3, 5, 300, 420, 128, 128, 48, 64, True, False),
+    (4, 2, 640, 900, 256, 256, 192, 128, True, True),
+    (5, 1, 640, 900, 256, 256, 256, 256, True, False),
+    (6, 1, 301, 427, 128, 128, 32, 256, True, True),        # width not a multiple of 4, ramp wider than the tile
+    (7, 1, 700, 1000, 256, 384, 96, 64, False, False),
+    (8, 1, 1300, 1800, 768, 768, 192, 128, True, True),
+    (9, 1, 1600, 2304, 1024, 1024, 64, 64, True, True),
+    (10, 1, 1500, 2200, 1024, 1024, 256, 256, False, False),
+    (11, 1, 1200, 2200, 2048, 2048, 128, 64, True, False),  # two 2176-px tiles, each nearly the whole canvas
+    (12, 1, 2100, 2500, 2048, 2048, 256, 64, False, True),
+    (13, 1, 64, 64, 2048, 2048, 256, 8, True, True),        # canvas << tile: 2304 -> 64 back-resize, 4x4 generic blocks
+    (14, 1, 80, 48, 2048, 2048, 256, 8, True, False),
+    (15, 1, 24, 1024, 2048, 2048, 256, 8, True, False),
+    (16, 1, 32, 32, 1024, 1024, 256, 8, True, False),
+]
+
+
+def wide_sampler(i: int):
+    return 2000 + i, 0.3 + 0.05 * (i % 8)

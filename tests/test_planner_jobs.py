@@ -23,7 +23,10 @@ def _ids(c):
     return f"{c[0]}-b{c[1]}-{c[3]}x{c[2]}-t{c[4]}-p{c[5]}-m{c[6]}-{'u' if c[7] else 'n'}"
 
 
-MMA_CASES = CASES + [("noise", 1, 320, 480, 256, 32, 8, True), ("noise", 1, 1200, 1600, 512, 32, 8, True)]
+MMA_CASES = CASES + [("noise", 1, 320, 480, 256, 32, 8, True), ("noise", 1, 1200, 1600, 512, 32, 8, True),
+                     # tensor-core crops staged with LDG (patch > the TMA boxes), one and two k-steps; two-k-step blend
+                     ("noise", 1, 500, 700, 128, 48, 8, True), ("noise", 1, 500, 700, 128, 96, 8, True),
+                     ("noise", 2, 400, 520, 128, 96, 8, True)]
 
 
 @pytest.mark.parametrize("path", [1, 2], ids=["fast", "mma"])
