@@ -16,7 +16,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libusdu_b200.so")
 
 # constants mirrored from include/usdu_b200.h (checked against the header in tests)
-ABI_VERSION = 10
+ABI_VERSION = 11
 ERR_INVALID = -1
 CANVAS_SLACK = 16
 PLAN_INFO_WORDS = 16
@@ -93,6 +93,8 @@ _SIGNATURES = {
     "usdu_graph_exec_destroy": (c_int, [c_void_p]),
     "usdu_pack_tiles_u8": (c_int, [c_void_p, c_void_p, c_int64, c_void_p]),
     "usdu_unpack_tiles_f32": (c_int, [c_void_p, c_void_p, c_int64, c_void_p]),
+    "usdu_png_sizes": (c_int, [c_int, c_int, c_int, POINTER(c_int64), POINTER(c_int64), POINTER(c_int64)]),
+    "usdu_png_base64_u8": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "usdu_t0_denoise": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_float, c_void_p]),
     "usdu_mask_scratch_bytes": (c_int64, [POINTER(c_int32), c_int]),
     "usdu_build_feather_masks": (c_int, [POINTER(c_int32), c_int, c_void_p, c_void_p, c_void_p]),
@@ -433,6 +435,17 @@ def pack_tiles_u8(src_ptr, dst_ptr, n, stream):
 
 def unpack_tiles_f32(src_ptr, dst_ptr, n, stream):
     _check(lib().usdu_unpack_tiles_f32(src_ptr, dst_ptr, n, stream), "usdu_unpack_tiles_f32")
+
+
+def png_sizes(H: int, W: int, C: int):
+    """-> (PNG bytes, base64 text bytes, device staging bytes) of one [H, W, C] frame (usdu_png_sizes)."""
+    png, text, staging = c_int64(), c_int64(), c_int64()
+    _check(lib().usdu_png_sizes(H, W, C, ctypes.byref(png), ctypes.byref(text), ctypes.byref(staging)), "usdu_png_sizes")
+    return png.value, text.value, staging.value
+
+
+def png_base64_u8(src_ptr, B, H, W, C, staging_ptr, text_ptr, stream):
+    _check(lib().usdu_png_base64_u8(src_ptr, B, H, W, C, staging_ptr, text_ptr, stream), "usdu_png_base64_u8")
 
 
 def t0_denoise(tiles_ptr, noise_ptr, out_ptr, n, frame, omd, stream):

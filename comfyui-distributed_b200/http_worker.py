@@ -1,6 +1,7 @@
 """Worker side of the reference's static-mode HTTP protocol (upscale/modes/static.py:191-314,
 upscale/worker_comms.py:16-188), so that a stock reference master can hand tiles to a worker whose tile step runs on
-this package's kernels (engine.WorkerJob).
+this package's kernels (engine.WorkerJob), and the worker side of its DistributedCollector (nodes/collector.py:84-119,
+`send_collector_batch`).
 
 Blocking HTTP on the caller's thread (ComfyUI's prompt executor) with the standard library; no event loop.  What goes on
 the wire is what the reference's worker sends: the job-ready poll, one `request_image` per tile, a heartbeat after every
@@ -9,6 +10,7 @@ the final chunk (or the empty completion signal).  Retry counts, delays and time
 """
 from __future__ import annotations
 
+import base64
 import io
 import json
 import os
@@ -17,7 +19,7 @@ import urllib.error
 import urllib.parse
 import urllib.request
 import uuid
-from typing import Callable, List, Optional, Sequence, Tuple
+from typing import Callable, Iterable, List, Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -30,6 +32,7 @@ SEND_RETRIES = 5                   # tile upload (worker_comms.py:88-104)
 TILE_SEND_TIMEOUT = 60.0           # utils/constants.py TILE_SEND_TIMEOUT
 CHUNK_HEADROOM = 1024 * 1024       # worker_comms.py:49
 TILE_OVERHEAD = 1024               # worker_comms.py:65
+COLLECTOR_TIMEOUT = 60.0           # one job_complete POST (collector.py:110-116)
 
 TileStep = Callable[[int], np.ndarray]
 """step(tile id) -> the processed tile of every frame, uint8 [B, ph, pw, 3] on the host."""
@@ -39,6 +42,22 @@ class HttpError(RuntimeError):
     def __init__(self, method: str, url: str, status: int, body: bytes):
         super().__init__(f"{method} {url}: HTTP {status}: {body[:200].decode('utf-8', 'replace')}")
         self.status = status
+
+
+# no proxy from the environment: the master is addressed directly, like the reference's aiohttp session
+_OPENER = urllib.request.build_opener(urllib.request.ProxyHandler({}))
+
+
+def _call(url: str, method: str, body: Optional[bytes] = None, ctype: Optional[str] = None,
+          timeout: float = STATUS_TIMEOUT) -> Tuple[int, bytes]:
+    """One blocking request -> (status, body); an HTTP error status is returned, a connection error raises."""
+    req = urllib.request.Request(url, data=body, method=method, headers={"Content-Type": ctype} if ctype else {})
+    try:
+        with _OPENER.open(req, timeout=timeout) as r:
+            return r.status, r.read()
+    except urllib.error.HTTPError as e:
+        with e:
+            return e.code, e.read()
 
 
 def encode_png(tile: np.ndarray) -> bytes:
@@ -90,20 +109,11 @@ class HttpStaticWorker:
         self.pulled: List[int] = []        # tile ids in processing order
         self.chunks = 0                    # tile uploads (multipart POSTs with tiles)
         self.times = {"request_s": 0.0, "step_s": 0.0, "encode_s": 0.0, "post_s": 0.0, "heartbeat_s": 0.0}
-        # no proxy from the environment: the master is addressed directly, like the reference's aiohttp session
-        self._opener = urllib.request.build_opener(urllib.request.ProxyHandler({}))
 
     # -- HTTP ---------------------------------------------------------------------------
     def _call(self, method: str, path: str, body: Optional[bytes] = None, ctype: Optional[str] = None,
               timeout: float = STATUS_TIMEOUT) -> Tuple[int, bytes]:
-        req = urllib.request.Request(self.master_url + path, data=body, method=method,
-                                     headers={"Content-Type": ctype} if ctype else {})
-        try:
-            with self._opener.open(req, timeout=timeout) as r:
-                return r.status, r.read()
-        except urllib.error.HTTPError as e:
-            with e:
-                return e.code, e.read()
+        return _call(self.master_url + path, method, body, ctype, timeout)
 
     def _post_json(self, path: str, obj: dict, timeout: float) -> Tuple[int, bytes]:
         return self._call("POST", path, json.dumps(obj).encode(), "application/json", timeout)
@@ -242,3 +252,74 @@ class HttpStaticWorker:
         self.send(pending, final=True)
         self.times["post_s"] += clock() - t0
         return True
+
+
+# --------------------------------------------------------------------------------------
+# DistributedCollector worker (nodes/collector.py:84-119 -> api/job_routes.py:273-343)
+# --------------------------------------------------------------------------------------
+def max_audio_payload_bytes() -> int:
+    return int(os.environ.get("COMFYUI_MAX_AUDIO_PAYLOAD_BYTES", str(256 * 1024 * 1024)))
+
+
+def encode_audio_payload(audio) -> Optional[dict]:
+    """The reference's audio envelope (utils/audio_payload.py:16-43): a float32 contiguous waveform's bytes in base64,
+    its shape, dtype "float32" and int(sample_rate) (44100 when that fails).  None for no audio or an empty waveform;
+    ValueError over COMFYUI_MAX_AUDIO_PAYLOAD_BYTES."""
+    import torch
+    if not isinstance(audio, dict):
+        return None
+    wave = audio.get("waveform")
+    if wave is None or not isinstance(wave, torch.Tensor) or wave.numel() == 0:
+        return None
+    try:
+        rate = int(audio.get("sample_rate", 44100))
+    except (TypeError, ValueError):
+        rate = 44100
+    w = wave.detach().to(device="cpu", dtype=torch.float32).contiguous()
+    data = w.numpy().tobytes()
+    limit = max_audio_payload_bytes()
+    if len(data) > limit:
+        raise ValueError(f"Audio payload too large: {len(data)} bytes exceeds {limit}.")
+    return {"sample_rate": rate, "shape": [int(d) for d in w.shape], "dtype": "float32",
+            "data": base64.b64encode(data).decode("ascii")}
+
+
+def collector_body(job_id: str, worker_id: str, batch_idx: int, text, is_last: bool,
+                   audio_json: Optional[bytes] = None) -> bytes:
+    """The JSON envelope of one image, built as bytes around the base64 text (which needs no escaping):
+    {"job_id", "worker_id", "batch_idx", "image": "data:image/png;base64,...", "is_last"[, "audio"]}."""
+    head = (b'{"job_id": ' + json.dumps(str(job_id)).encode() + b', "worker_id": ' + json.dumps(str(worker_id)).encode()
+            + b', "batch_idx": ' + str(int(batch_idx)).encode() + b', "image": "data:image/png;base64,')
+    tail = b'", "is_last": ' + (b"true" if is_last else b"false")
+    if audio_json is not None:
+        tail += b', "audio": ' + audio_json
+    return b"".join((head, text, tail, b"}"))
+
+
+def send_collector_batch(master_url: str, job_id: str, worker_id: str, count: int, texts: Iterable, audio=None,
+                         post_times: Optional[List[float]] = None) -> int:
+    """POST `count` images to {master_url}/distributed/job_complete, one per image in batch order, `is_last` on the
+    last, the audio envelope beside it.  `texts` yields each image's base64 PNG text (bytes-like) and is only advanced
+    after the previous image was posted.  Any status >= 400 or connection error raises, with no retry, as the
+    reference re-raises.  count = 0 sends nothing.  -> images sent."""
+    if count == 0:
+        return 0
+    audio_payload = encode_audio_payload(audio)
+    audio_json = None if audio_payload is None else json.dumps(audio_payload).encode()
+    url = master_url + "/distributed/job_complete"
+    sent = 0
+    for text in texts:
+        if sent >= count:
+            raise ValueError(f"more than {count} images to send")
+        last = sent == count - 1
+        body = collector_body(job_id, worker_id, sent, text, last, audio_json if last else None)
+        t0 = time.perf_counter()
+        status, reply = _call(url, "POST", body, "application/json", COLLECTOR_TIMEOUT)
+        if post_times is not None:
+            post_times.append(time.perf_counter() - t0)
+        if status >= 400:
+            raise HttpError("POST", url, status, reply)
+        sent += 1
+    if sent != count:
+        raise ValueError(f"{sent} of {count} images encoded")
+    return sent

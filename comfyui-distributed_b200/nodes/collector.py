@@ -6,6 +6,11 @@ to one NCCL all-gather of u8 images and rank 0 assembles the result in the refer
 order: master's images first (kept at full fp32 precision, collector.py:276), then each
 enabled worker's images (which went through the truncating u8 cast, collector.py:95-98),
 then unexpected workers sorted by id (collector.py:193-236).  Audio stays in Python.
+
+Started by the reference's orchestrator as an HTTP worker (no torch.distributed peers), the node sends its images to
+the reference's master as that worker does: one job_complete POST per image with a level-0 PNG in base64
+(http_worker.send_collector_batch).  The cast, the PNG layout and the base64 text are computed on the GPU
+(usdu_png_base64_u8); only the finished text goes to the host.
 """
 from __future__ import annotations
 
@@ -14,7 +19,10 @@ import json
 import torch
 
 from .. import dist as usdu_dist
+from .. import http_worker
 from ..casts import reference_f32
+
+PNG_TEXT_BUDGET = 64 << 20    # pinned host bytes for one group of frames' base64 text (at least one frame)
 
 
 def _native_pack(images: torch.Tensor) -> torch.Tensor:
@@ -37,6 +45,53 @@ def _native_unpack(q: torch.Tensor) -> torch.Tensor:
     with torch.cuda.device(q.device):
         nat.unpack_tiles_f32(q.data_ptr(), out.data_ptr(), q.numel(), torch.cuda.current_stream().cuda_stream)
     return out
+
+
+_text_pool = None
+
+
+def _native_png_b64(q: torch.Tensor):
+    """u8 CUDA frames [B,H,W,C] -> each frame's base64 PNG text in batch order (usdu_png_base64_u8).  Frames are encoded
+    in groups whose text fits PNG_TEXT_BUDGET; a group's text is copied to pinned host memory once.  Each item is a
+    memoryview into that buffer, valid until the next item is requested."""
+    global _text_pool
+    from .. import _native as nat
+    from ..engine import _PinnedPool
+    B, H, W, C = (int(v) for v in q.shape)
+    if B == 0:
+        return
+    _, text_len, staging_len = nat.png_sizes(H, W, C)
+    group = max(1, min(B, PNG_TEXT_BUDGET // text_len))
+    q = q.contiguous()
+    if _text_pool is None:
+        _text_pool = _PinnedPool(keep=1, shapes=2)
+    host = _text_pool.get((group * text_len,), torch.uint8)
+    with torch.cuda.device(q.device):
+        stream = torch.cuda.current_stream()
+        staging = torch.empty(group * staging_len, dtype=torch.uint8, device=q.device)
+        text = torch.empty(group * text_len, dtype=torch.uint8, device=q.device)
+        view = memoryview(host.numpy())
+        for b0 in range(0, B, group):
+            n = min(group, B - b0)
+            nat.png_base64_u8(q[b0].data_ptr(), n, H, W, C, staging.data_ptr(), text.data_ptr(), stream.cuda_stream)
+            host[:n * text_len].copy_(text[:n * text_len], non_blocking=True)
+            stream.synchronize()
+            for i in range(n):
+                yield view[i * text_len:(i + 1) * text_len]
+
+
+def send_to_master(images: torch.Tensor, audio, multi_job_id: str, master_url: str, worker_id: str,
+                   pack=_native_pack, encode=_native_png_b64, post_times=None) -> int:
+    """The reference worker's send_batch_to_master (collector.py:84-119): B = 0 sends nothing; a frame PIL cannot write
+    as PNG (C other than 2, 3 or 4) raises TypeError before any request, as Image.fromarray does.  -> images sent."""
+    B = int(images.shape[0]) if images.ndim >= 1 else 0
+    if B == 0:
+        return 0
+    if images.ndim != 4 or images.shape[-1] not in (2, 3, 4):
+        raise TypeError(f"DistributedCollector: cannot send frames of shape {tuple(images.shape[1:])} as PNG "
+                        "(2, 3 or 4 channels)")
+    return http_worker.send_collector_batch(master_url, multi_job_id, worker_id, B, encode(pack(images)), audio,
+                                            post_times)
 
 
 def collect_images(images: torch.Tensor, enabled_worker_ids, worker_id: str, delegate_only: bool = False,
@@ -84,6 +139,9 @@ def combine_audio(pieces, empty_audio):
 
 class DistributedCollectorNode:
     EMPTY_AUDIO = {"waveform": torch.zeros(1, 2, 1), "sample_rate": 44100}
+    # the HTTP worker's cast (IMAGE -> u8 frames) and encoder (u8 frames -> base64 PNG texts)
+    pack = staticmethod(_native_pack)
+    encode = staticmethod(_native_png_b64)
 
     @classmethod
     def INPUT_TYPES(s):
@@ -120,15 +178,11 @@ class DistributedCollectorNode:
             return (images, audio if audio is not None else empty_audio)
         rank, world = usdu_dist.dist_info()
         enabled = [str(w) for w in json.loads(enabled_worker_ids)]
-        if world == 1:  # no participants besides the master (collector.py:255-256)
-            if is_worker:
-                # started as an HTTP worker of the reference's orchestrator: there is no torch.distributed peer to send the
-                # batch to, and the reference's HTTP collection is not part of this package -- say so instead of dropping it
-                import warnings
-                warnings.warn("DistributedCollector (CUDA tile path): running as an HTTP worker of the reference's orchestrator is not "
-                              "supported (launch one rank per GPU with torch.distributed); this worker's images stay local.",
-                              RuntimeWarning, stacklevel=2)
-            return (images, audio if audio is not None else empty_audio)
+        if world == 1:
+            if is_worker:   # an HTTP worker of the reference's orchestrator: send to its master (collector.py:239-243)
+                send_to_master(images, audio, multi_job_id, master_url, worker_id, pack=self.pack, encode=self.encode)
+                return (images, audio if audio is not None else self.EMPTY_AUDIO)
+            return (images, audio if audio is not None else empty_audio)   # no participants (collector.py:255-256)
         wid = worker_id if (worker_id or rank == 0) else f"rank{rank}"
         if not enabled:  # SPMD launch without the reference's orchestrator: every rank is enabled
             enabled = [f"rank{r}" for r in range(1, world)]

@@ -35,7 +35,7 @@ extern "C" {
 #pragma GCC visibility push(default) /* the library itself is built with -fvisibility=hidden */
 #endif
 
-#define USDU_ABI_VERSION 10
+#define USDU_ABI_VERSION 11
 
 typedef enum usdu_status {
     USDU_OK = 0,
@@ -282,6 +282,23 @@ int usdu_gather_canvas(const uint8_t* const* slab_canvas_dev, const int32_t* sla
 int usdu_pack_tiles_u8(const float* src_dev, uint8_t* dst_dev, int64_t n, void* stream);
 /* receiving side of the transport: dst[i] = src[i] / 255.0f (api/job_routes.py:104-132) */
 int usdu_unpack_tiles_f32(const uint8_t* src_dev, float* dst_dev, int64_t n, void* stream);
+
+/* Collector worker transport (nodes/collector.py:84-119): each u8 frame [H, W, C] as the base64 text of one PNG,
+ * what the reference's worker POSTs to /distributed/job_complete.  The PNG is stored (deflate level 0, filter None),
+ * its bytes fixed by this layout (tests/png_model.py png_stored_b64 states it in numpy):
+ *   8-byte signature; IHDR (W, H, depth 8, colour type 4 / 2 / 6 for C = 2 / 3 / 4, compression, filter, interlace 0);
+ *   the raw stream R = per row a filter byte 0 and the row's W*C bytes, |R| = H*(1 + W*C), cut into stored deflate
+ *   blocks of 65535 bytes (the last shorter); block k alone in IDAT chunk k, whose data is [78 01 if k == 0] +
+ *   [BFINAL | BTYPE 00] + LEN (le16) + NLEN (le16) + the block; one IDAT chunk holding the big-endian Adler-32 of R;
+ *   IEND.  Text: standard base64 alphabet, '=' padding, no line breaks, no terminator.
+ * usdu_png_sizes: for one frame, the PNG length, the text length and the device staging bytes; USDU_ERR_INVALID
+ * unless C is 2, 3 or 4 and H, W >= 1.
+ * usdu_png_base64_u8: src_dev = B contiguous u8 frames [H, W, C]; staging_dev = B * staging bytes (16-byte aligned,
+ * scratch); frame b's text goes to text_dev + b * text length (text_dev 4-byte aligned).  Three launches on `stream`,
+ * no host synchronisation.  B <= 65535. */
+int usdu_png_sizes(int H, int W, int C, int64_t* png_len, int64_t* text_len, int64_t* staging_bytes);
+int usdu_png_base64_u8(const uint8_t* src_dev, int B, int H, int W, int C, uint8_t* staging_dev, char* text_dev,
+                       void* stream);
 
 /* TEST DOUBLE, not part of the reference path: the deterministic T0 sampler stand-in used by the
  * parity tests and bench.py (BASELINE.md section 3) as one fused pass,
