@@ -16,7 +16,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libusdu_b200.so")
 
 # constants mirrored from include/usdu_b200.h (checked against the header in tests)
-ABI_VERSION = 11
+ABI_VERSION = 12
 ERR_INVALID = -1
 CANVAS_SLACK = 16
 PLAN_INFO_WORDS = 16
@@ -95,6 +95,7 @@ _SIGNATURES = {
     "usdu_unpack_tiles_f32": (c_int, [c_void_p, c_void_p, c_int64, c_void_p]),
     "usdu_png_sizes": (c_int, [c_int, c_int, c_int, POINTER(c_int64), POINTER(c_int64), POINTER(c_int64)]),
     "usdu_png_base64_u8": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "usdu_png_decode_u8": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "usdu_t0_denoise": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_float, c_void_p]),
     "usdu_mask_scratch_bytes": (c_int64, [POINTER(c_int32), c_int]),
     "usdu_build_feather_masks": (c_int, [POINTER(c_int32), c_int, c_void_p, c_void_p, c_void_p]),
@@ -446,6 +447,15 @@ def png_sizes(H: int, W: int, C: int):
 
 def png_base64_u8(src_ptr, B, H, W, C, staging_ptr, text_ptr, stream):
     _check(lib().usdu_png_base64_u8(src_ptr, B, H, W, C, staging_ptr, text_ptr, stream), "usdu_png_base64_u8")
+
+
+PNG_DESC_WORDS = 8
+PNG_MAX_ROW_BYTES = 14336
+
+
+def png_decode_u8(src_ptr, segs_ptr, n_segs, descs_ptr, n, max_row_bytes, dst_ptr, stream):
+    _check(lib().usdu_png_decode_u8(src_ptr, segs_ptr, n_segs, descs_ptr, n, max_row_bytes, dst_ptr, stream),
+           "usdu_png_decode_u8")
 
 
 def t0_denoise(tiles_ptr, noise_ptr, out_ptr, n, frame, omd, stream):

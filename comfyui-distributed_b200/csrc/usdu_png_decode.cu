@@ -1,0 +1,170 @@
+// usdu_png_decode.cu -- PNG tiles posted by static-mode workers -> u8 RGB frames at their payload offsets, on the device.
+//
+// A worker of the reference's protocol posts each processed tile as a PIL PNG at compress_level=0: one IHDR, IDAT
+// chunks holding a zlib stream of STORED deflate blocks, and rows filtered per row with None / Sub / Up / Avg / Paeth.
+// The master's route handler validates every file on the host (http_master.parse_png) and records, per frame, the
+// segments of the uploaded bytes that hold the filtered stream R (per row: the filter byte, then the row's W*C bytes),
+// skipping chunk framing, the zlib header and the stored-block headers.  A stream with compressed blocks is inflated on
+// the host and its R uploaded as one segment.  What is left on the device is byte moving plus PNG un-filtering, and the
+// conversion PIL's convert("RGB") does: grey (C = 1) replicated, grey+alpha (2) and RGBA (4) drop the alpha.
+//
+// Un-filtering is serial along a row (Sub, Avg, Paeth read the pixel to the left) and down the rows (Up, Avg, Paeth read
+// the row above), so one CTA per frame runs a CHUNKED WAVEFRONT: warp w owns rows w, w + kWarps, ...; a row is cut into
+// chunks of 32 pixels, one pixel per lane; chunk k of row r starts once row r - 1 has published chunk k.  Decoded rows
+// live in a shared-memory ring of kWarps rows (warp w's slot), so before a warp overwrites chunk k of its slot it waits
+// until the row after the previous occupant has read it (chunk k + 1 too: Paeth's upper-left pixel).  Progress counters
+// in shared memory (row * chunks + chunks published) order the warps.
+//   None, Up  lane-parallel;  Sub  a warp scan per channel, mod 256, carried across chunks;
+//   Avg, Paeth  serial per channel inside the chunk (lanes 0..C-1), in place in the ring slot.
+#include "usdu_common.cuh"
+
+namespace usdu {
+namespace {
+
+constexpr int kDecWarps = 16;
+constexpr int kDecThreads = kDecWarps * 32;
+constexpr int kChunk = 32;                        // pixels per chunk, one per lane
+
+__device__ __forceinline__ int ld_volatile(const int* p) { return *reinterpret_cast<const volatile int*>(p); }
+
+__device__ __forceinline__ void wait_progress(const int* prog, int need) {
+    if ((threadIdx.x & 31) == 0)
+        while (ld_volatile(prog) < need) {
+        }
+    __syncwarp();
+    __threadfence_block();
+}
+
+// The bytes of R from raw position q on: each lane walks its own segment cursor forward (positions only grow per lane).
+struct SegCursor {
+    const int64_t* segs;    // this frame's segments: (src offset, raw start) pairs
+    int n;                  // segments of this frame
+    int64_t raw_len;        // |R|
+    int s;                  // current segment
+    __device__ __forceinline__ uint32_t byte(const uint8_t* src, int64_t q) {
+        while (s + 1 < n && segs[2 * (s + 1) + 1] <= q) ++s;
+        return src[segs[2 * s] + (q - segs[2 * s + 1])];
+    }
+};
+
+__device__ __forceinline__ uint32_t paeth(uint32_t a, uint32_t b, uint32_t c) {
+    const int p = (int)a + (int)b - (int)c;
+    const int pa = abs(p - (int)a), pb = abs(p - (int)b), pc = abs(p - (int)c);
+    return (pa <= pb && pa <= pc) ? a : (pb <= pc ? b : c);
+}
+
+__global__ void __launch_bounds__(kDecThreads) png_decode_kernel(const uint8_t* __restrict__ src,
+                                                                 const int64_t* __restrict__ segs, int64_t n_segs,
+                                                                 const int64_t* __restrict__ descs,
+                                                                 uint8_t* __restrict__ dst) {
+    extern __shared__ __align__(16) uint8_t ring[];
+    __shared__ int prog[kDecWarps];
+    const int64_t* d = descs + (int64_t)blockIdx.x * USDU_PNG_DESC_WORDS;
+    const int64_t seg0 = d[0], nseg = d[1];
+    const int H = (int)d[2], W = (int)d[3], C = (int)d[4];
+    uint8_t* out = dst + d[5];
+    if (seg0 < 0 || nseg < 1 || seg0 + nseg > n_segs) return;          // the launcher checked the host tables
+    const int n = W * C;                                                // bytes of a decoded row
+    const int nch = (W + kChunk - 1) / kChunk;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (threadIdx.x < kDecWarps) prog[threadIdx.x] = 0;
+    __syncthreads();
+
+    SegCursor cur{segs + 2 * seg0, (int)nseg, (int64_t)H * (n + 1), 0};
+    uint8_t* mine = ring + warp * n;
+    for (int r = warp; r < H; r += kDecWarps) {
+        const uint8_t* above = r > 0 ? ring + ((r - 1) % kDecWarps) * n : nullptr;
+        const int* prog_above = &prog[(r - 1 + kDecWarps) % kDecWarps];
+        const int* prog_next = &prog[(warp + 1) % kDecWarps];           // the row after this slot's previous occupant
+        const int64_t row_raw = (int64_t)r * (n + 1);
+        const uint32_t filt = __shfl_sync(0xffffffffu, lane == 0 ? cur.byte(src, row_raw) : 0u, 0);
+        uint32_t carry[4] = {0, 0, 0, 0};                               // Sub: last decoded pixel of the previous chunk
+        for (int k = 0; k < nch; ++k) {
+            const int x = k * kChunk + lane;
+            const int cnt = min(kChunk, W - k * kChunk);
+            // the slot's previous occupant (row r - kWarps) must have been read up to chunk k + 1 by row r - kWarps + 1
+            if (r >= kDecWarps) wait_progress(prog_next, (r - kDecWarps + 1) * nch + min(k + 2, nch));
+            if (r > 0 && (filt >= 2)) wait_progress(prog_above, (r - 1) * nch + k + 1);
+            uint32_t v[4] = {0, 0, 0, 0};
+            if (lane < cnt) {
+#pragma unroll
+                for (int c = 0; c < 4; ++c)
+                    if (c < C) v[c] = cur.byte(src, row_raw + 1 + (int64_t)x * C + c);
+            }
+            if (filt == 1) {                                            // Sub: inclusive scan over the chunk, per channel
+#pragma unroll
+                for (int c = 0; c < 4; ++c) {
+                    uint32_t s = v[c];
+#pragma unroll
+                    for (int o = 1; o < 32; o <<= 1) {
+                        const uint32_t t = __shfl_up_sync(0xffffffffu, s, o);
+                        if (lane >= o) s += t;
+                    }
+                    v[c] = (s + carry[c]) & 0xffu;
+                    carry[c] = __shfl_sync(0xffffffffu, v[c], cnt - 1);
+                }
+            } else if (filt == 2 && lane < cnt && r > 0) {              // Up
+#pragma unroll
+                for (int c = 0; c < 4; ++c)
+                    if (c < C) v[c] = (v[c] + above[x * C + c]) & 0xffu;
+            }
+            if (lane < cnt) {
+#pragma unroll
+                for (int c = 0; c < 4; ++c)
+                    if (c < C) mine[x * C + c] = (uint8_t)v[c];
+            }
+            __syncwarp();
+            if (filt >= 3 && lane < C) {                                // Avg, Paeth: serial per channel, in place
+                const int c = lane;
+                uint32_t left = k > 0 ? mine[(k * kChunk - 1) * C + c] : 0u;
+                uint32_t ul = (k > 0 && r > 0) ? above[(k * kChunk - 1) * C + c] : 0u;
+                for (int i = 0; i < cnt; ++i) {
+                    const int o = (k * kChunk + i) * C + c;
+                    const uint32_t up = r > 0 ? above[o] : 0u;
+                    const uint32_t f = mine[o];
+                    const uint32_t pred = filt == 3 ? ((left + up) >> 1) : paeth(left, up, ul);
+                    left = (f + pred) & 0xffu;
+                    mine[o] = (uint8_t)left;
+                    ul = up;
+                }
+            }
+            __syncwarp();
+            if (lane < cnt) {                                           // convert("RGB") and store
+                const uint8_t* p = mine + x * C;
+                uint8_t* q = out + ((int64_t)r * W + x) * 3;
+                const uint8_t c0 = p[0];
+                q[0] = c0;
+                q[1] = C >= 3 ? p[1] : c0;
+                q[2] = C >= 3 ? p[2] : c0;
+            }
+            __threadfence_block();
+            __syncwarp();
+            if (lane == 0) *reinterpret_cast<volatile int*>(&prog[warp]) = r * nch + k + 1;
+        }
+    }
+}
+
+}  // namespace
+}  // namespace usdu
+
+using namespace usdu;
+
+extern "C" {
+
+int usdu_png_decode_u8(const uint8_t* src_dev, const int64_t* segs_dev, int64_t n_segs, const int64_t* descs_dev,
+                       int n, int max_row_bytes, uint8_t* dst_dev, void* stream) {
+    USDU_REQUIRE(n >= 0, "usdu_png_decode_u8: %d frames", n);
+    if (n == 0) return USDU_OK;
+    USDU_REQUIRE(src_dev && segs_dev && descs_dev && dst_dev, "usdu_png_decode_u8: null pointer");
+    USDU_REQUIRE(n_segs >= 1, "usdu_png_decode_u8: no segments");
+    USDU_REQUIRE(max_row_bytes >= 1 && max_row_bytes <= USDU_PNG_MAX_ROW_BYTES,
+                 "usdu_png_decode_u8: row bytes %d outside [1, %d]", max_row_bytes, USDU_PNG_MAX_ROW_BYTES);
+    const size_t smem = (size_t)kDecWarps * (size_t)max_row_bytes;
+    int r = raise_smem_limit((const void*)png_decode_kernel, smem);
+    if (r != USDU_OK) return r;
+    png_decode_kernel<<<n, kDecThreads, smem, (cudaStream_t)stream>>>(src_dev, segs_dev, n_segs, descs_dev, dst_dev);
+    USDU_CUDA(cudaGetLastError());
+    return USDU_OK;
+}
+
+}  // extern "C"

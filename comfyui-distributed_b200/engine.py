@@ -929,6 +929,16 @@ class WorkerJob:
         self.times["tiles"] += 1
         return host.numpy()
 
+    def step_device(self, tile_id: int):
+        """Process tile `tile_id` into this canvas only (the master of HTTP workers: its tiles never leave the device).
+        Enqueued on the current stream, no host synchronisation."""
+        tile_id = int(tile_id)
+        if not 0 <= tile_id < len(self.plan.tiles):
+            raise ValueError(f"tile id {tile_id} is outside this job's {len(self.plan.tiles)} tiles")
+        with torch.cuda.device(self.device):
+            run_progressive(self.canvas, [tile_id], self.denoiser)
+        self.times["tiles"] += 1
+
 
 # --------------------------------------------------------------------------------------
 # host-tensor path: H2D, compute and D2H overlapped band by band

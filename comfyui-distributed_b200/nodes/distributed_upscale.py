@@ -25,6 +25,7 @@ import os
 import torch
 
 from .. import dist as usdu_dist
+from .. import http_master
 from ..casts import reference_f32
 from ..denoise import ComfySampler
 from ..engine import WorkerJob, upscale_host, upscale_single
@@ -132,6 +133,24 @@ class UltimateSDUpscaleDistributed:
             worker.run(job.step)
             self.last_stats.update(pulled=list(worker.pulled), chunks=worker.chunks)
             return (upscaled_image,)
+        if multi_job_id and not is_worker and world == 1 and json.loads(enabled_worker_ids) and http_master.serving():
+            # This process serves the reference's USDU routes (http_master.py): be the static-mode master of the HTTP
+            # workers (static.py:371-570) -- own tiles from the shared queue on this GPU, worker PNG tiles decoded on
+            # the GPU as they arrive, one composite at the end.
+            _, H, W, _ = upscaled_image.shape
+            denoiser = self._make_denoiser(model, positive, negative, vae, seed, steps, cfg, sampler_name, scheduler,
+                                           denoise, tiled_decode, (W, H))
+            job = WorkerJob(upscaled_image, denoiser, tile_width, tile_height, padding, mask_blur, force_uniform_tiles,
+                            device=dev)
+            master = http_master.HttpStaticMaster(job, multi_job_id, [str(w) for w in json.loads(enabled_worker_ids)])
+            out = master.run()
+            self.last_stats.update(master.stats, assignment=master.assignment())
+            if not upscaled_image.is_cuda:
+                pinned = torch.empty(out.shape, dtype=out.dtype, pin_memory=True)
+                pinned.copy_(out, non_blocking=True)
+                torch.cuda.current_stream(dev).synchronize()
+                out = pinned
+            return (out,)
         if self.semantics not in ("static", "exact"):
             raise ValueError(f"semantics must be 'static' or 'exact', got {self.semantics!r}")
         exact = distributed and self.semantics == "exact"

@@ -35,7 +35,7 @@ extern "C" {
 #pragma GCC visibility push(default) /* the library itself is built with -fvisibility=hidden */
 #endif
 
-#define USDU_ABI_VERSION 11
+#define USDU_ABI_VERSION 12
 
 typedef enum usdu_status {
     USDU_OK = 0,
@@ -299,6 +299,22 @@ int usdu_unpack_tiles_f32(const uint8_t* src_dev, float* dst_dev, int64_t n, voi
 int usdu_png_sizes(int H, int W, int C, int64_t* png_len, int64_t* text_len, int64_t* staging_bytes);
 int usdu_png_base64_u8(const uint8_t* src_dev, int B, int H, int W, int C, uint8_t* staging_dev, char* text_dev,
                        void* stream);
+
+/* Master side of the static-mode transport (upscale/payload_parsers.py:32-36): the level-0 PNG tiles workers post,
+ * decoded to u8 RGB frames in one launch, one CTA per frame.  The host validates each file and cuts it into segments:
+ * runs of the uploaded bytes that, in order, form the frame's filtered stream R (per row a filter byte 0..4, then the
+ * row's W*C bytes; |R| = H*(1 + W*C)), chunk framing, zlib header and stored-block headers left out.
+ * segs_dev: n_segs (src offset, raw start) int64 pairs -- the segment starting at R[raw start] lies at
+ *   src_dev + src offset and runs to the next segment's raw start (the frame's last one to |R|); a frame's first raw
+ *   start is 0.
+ * descs_dev: n descriptors of USDU_PNG_DESC_WORDS int64: first segment, segment count, H, W, C (1 grey, 2 grey+alpha,
+ *   3 RGB, 4 RGBA), byte offset of the frame's [H, W, 3] u8 output in dst_dev, 0, 0.
+ * The rows are un-filtered (None / Sub / Up / Avg / Paeth) and converted as PIL's convert("RGB"): grey replicated,
+ * alpha dropped.  max_row_bytes >= every frame's W*C and <= USDU_PNG_MAX_ROW_BYTES (shared memory holds 16 rows). */
+#define USDU_PNG_DESC_WORDS 8
+#define USDU_PNG_MAX_ROW_BYTES 14336
+int usdu_png_decode_u8(const uint8_t* src_dev, const int64_t* segs_dev, int64_t n_segs, const int64_t* descs_dev,
+                       int n, int max_row_bytes, uint8_t* dst_dev, void* stream);
 
 /* TEST DOUBLE, not part of the reference path: the deterministic T0 sampler stand-in used by the
  * parity tests and bench.py (BASELINE.md section 3) as one fused pass,
