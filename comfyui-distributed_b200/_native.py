@@ -16,7 +16,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libusdu_b200.so")
 
 # constants mirrored from include/usdu_b200.h (checked against the header in tests)
-ABI_VERSION = 12
+ABI_VERSION = 13
 ERR_INVALID = -1
 CANVAS_SLACK = 16
 PLAN_INFO_WORDS = 16
@@ -96,6 +96,8 @@ _SIGNATURES = {
     "usdu_png_sizes": (c_int, [c_int, c_int, c_int, POINTER(c_int64), POINTER(c_int64), POINTER(c_int64)]),
     "usdu_png_base64_u8": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "usdu_png_decode_u8": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    "usdu_png_decode_warps": (c_int, [c_int]),
+    "usdu_gather_unpack_f32": (c_int, [c_void_p, c_int, c_int64, c_void_p, c_void_p]),
     "usdu_t0_denoise": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_float, c_void_p]),
     "usdu_mask_scratch_bytes": (c_int64, [POINTER(c_int32), c_int]),
     "usdu_build_feather_masks": (c_int, [POINTER(c_int32), c_int, c_void_p, c_void_p, c_void_p]),
@@ -450,12 +452,25 @@ def png_base64_u8(src_ptr, B, H, W, C, staging_ptr, text_ptr, stream):
 
 
 PNG_DESC_WORDS = 8
-PNG_MAX_ROW_BYTES = 14336
+PNG_MAX_ROW_BYTES = 65536      # 16,384 px (ComfyUI's MAX_RESOLUTION) at 4 channels
 
 
 def png_decode_u8(src_ptr, segs_ptr, n_segs, descs_ptr, n, max_row_bytes, dst_ptr, stream):
     _check(lib().usdu_png_decode_u8(src_ptr, segs_ptr, n_segs, descs_ptr, n, max_row_bytes, dst_ptr, stream),
            "usdu_png_decode_u8")
+
+
+def png_decode_warps(max_row_bytes: int) -> int:
+    """Ring depth (= warps per CTA) usdu_png_decode_u8 uses for rows of up to max_row_bytes on the current device."""
+    r = lib().usdu_png_decode_warps(max_row_bytes)
+    if r < 0:
+        _check(r, "usdu_png_decode_warps")
+    return r
+
+
+def gather_unpack_f32(frame_ptrs_dev, n, frame_elems, dst_ptr, stream):
+    """frame_ptrs_dev: device array of n u8 frame addresses; dst: device or pinned host memory (usdu_gather_unpack_f32)."""
+    _check(lib().usdu_gather_unpack_f32(frame_ptrs_dev, n, frame_elems, dst_ptr, stream), "usdu_gather_unpack_f32")
 
 
 def t0_denoise(tiles_ptr, noise_ptr, out_ptr, n, frame, omd, stream):

@@ -1,4 +1,5 @@
-// usdu_png_decode.cu -- PNG tiles posted by static-mode workers -> u8 RGB frames at their payload offsets, on the device.
+// usdu_png_decode.cu -- PNGs posted by HTTP workers (static-mode tiles, collector images) -> u8 RGB frames, on the device;
+// and the collector master's gather of decoded frames into its fp32 result.
 //
 // A worker of the reference's protocol posts each processed tile as a PIL PNG at compress_level=0: one IHDR, IDAT
 // chunks holding a zlib stream of STORED deflate blocks, and rows filtered per row with None / Sub / Up / Avg / Paeth.
@@ -9,11 +10,14 @@
 // conversion PIL's convert("RGB") does: grey (C = 1) replicated, grey+alpha (2) and RGBA (4) drop the alpha.
 //
 // Un-filtering is serial along a row (Sub, Avg, Paeth read the pixel to the left) and down the rows (Up, Avg, Paeth read
-// the row above), so one CTA per frame runs a CHUNKED WAVEFRONT: warp w owns rows w, w + kWarps, ...; a row is cut into
+// the row above), so one CTA per frame runs a CHUNKED WAVEFRONT: warp w of D owns rows w, w + D, ...; a row is cut into
 // chunks of 32 pixels, one pixel per lane; chunk k of row r starts once row r - 1 has published chunk k.  Decoded rows
-// live in a shared-memory ring of kWarps rows (warp w's slot), so before a warp overwrites chunk k of its slot it waits
+// live in a shared-memory ring of D rows (warp w's slot), so before a warp overwrites chunk k of its slot it waits
 // until the row after the previous occupant has read it (chunk k + 1 too: Paeth's upper-left pixel).  Progress counters
-// in shared memory (row * chunks + chunks published) order the warps.
+// in shared memory (row * chunks + chunks published) order the warps.  The ring depth D, and with it the warps per CTA,
+// is min(16, opt-in shared memory / max_row_bytes): 16 up to 14,524-byte rows (tiles), 3 at 65,536 (16,384 RGBA px).
+// Any D >= 2 is deadlock-free: the warp a row waits on (the row above, or the row after its slot's previous occupant)
+// only ever waits on rows further up.
 //   None, Up  lane-parallel;  Sub  a warp scan per channel, mod 256, carried across chunks;
 //   Avg, Paeth  serial per channel inside the chunk (lanes 0..C-1), in place in the ring slot.
 #include "usdu_common.cuh"
@@ -21,8 +25,9 @@
 namespace usdu {
 namespace {
 
-constexpr int kDecWarps = 16;
+constexpr int kDecWarps = 16;                     // the deepest ring; the launch picks D <= kDecWarps warps
 constexpr int kDecThreads = kDecWarps * 32;
+constexpr int kDecMinWarps = 2;
 constexpr int kChunk = 32;                        // pixels per chunk, one per lane
 
 __device__ __forceinline__ int ld_volatile(const int* p) { return *reinterpret_cast<const volatile int*>(p); }
@@ -66,24 +71,25 @@ __global__ void __launch_bounds__(kDecThreads) png_decode_kernel(const uint8_t* 
     if (seg0 < 0 || nseg < 1 || seg0 + nseg > n_segs) return;          // the launcher checked the host tables
     const int n = W * C;                                                // bytes of a decoded row
     const int nch = (W + kChunk - 1) / kChunk;
+    const int D = blockDim.x >> 5;                                      // ring depth = warps
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    if (threadIdx.x < kDecWarps) prog[threadIdx.x] = 0;
+    if (threadIdx.x < D) prog[threadIdx.x] = 0;
     __syncthreads();
 
     SegCursor cur{segs + 2 * seg0, (int)nseg, (int64_t)H * (n + 1), 0};
     uint8_t* mine = ring + warp * n;
-    for (int r = warp; r < H; r += kDecWarps) {
-        const uint8_t* above = r > 0 ? ring + ((r - 1) % kDecWarps) * n : nullptr;
-        const int* prog_above = &prog[(r - 1 + kDecWarps) % kDecWarps];
-        const int* prog_next = &prog[(warp + 1) % kDecWarps];           // the row after this slot's previous occupant
+    for (int r = warp; r < H; r += D) {
+        const uint8_t* above = r > 0 ? ring + ((r - 1) % D) * n : nullptr;
+        const int* prog_above = &prog[(r - 1 + D) % D];
+        const int* prog_next = &prog[(warp + 1) % D];                   // the row after this slot's previous occupant
         const int64_t row_raw = (int64_t)r * (n + 1);
         const uint32_t filt = __shfl_sync(0xffffffffu, lane == 0 ? cur.byte(src, row_raw) : 0u, 0);
         uint32_t carry[4] = {0, 0, 0, 0};                               // Sub: last decoded pixel of the previous chunk
         for (int k = 0; k < nch; ++k) {
             const int x = k * kChunk + lane;
             const int cnt = min(kChunk, W - k * kChunk);
-            // the slot's previous occupant (row r - kWarps) must have been read up to chunk k + 1 by row r - kWarps + 1
-            if (r >= kDecWarps) wait_progress(prog_next, (r - kDecWarps + 1) * nch + min(k + 2, nch));
+            // the slot's previous occupant (row r - D) must have been read up to chunk k + 1 by row r - D + 1
+            if (r >= D) wait_progress(prog_next, (r - D + 1) * nch + min(k + 2, nch));
             if (r > 0 && (filt >= 2)) wait_progress(prog_above, (r - 1) * nch + k + 1);
             uint32_t v[4] = {0, 0, 0, 0};
             if (lane < cnt) {
@@ -144,6 +150,47 @@ __global__ void __launch_bounds__(kDecThreads) png_decode_kernel(const uint8_t* 
     }
 }
 
+// frame i of n: dst[i * frame_elems + e] = frames[i][e] / 255 (dequant_u8_fast, bit-identical to __fdiv_rn).  Each
+// thread writes 4 consecutive floats with one 16-byte store, from the frame's first 16-byte-aligned output element on
+// (its `head` elements before that are written singly), so a dst in mapped host memory gets whole 128-byte lines.
+__global__ void __launch_bounds__(kThreads) gather_unpack_kernel(const uint8_t* const* __restrict__ frames, int n,
+                                                                 int64_t frame_elems, float* __restrict__ dst) {
+    const int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int f = blockIdx.y; f < n; f += gridDim.y) {
+        const uint8_t* src = frames[f];
+        float* out = dst + (int64_t)f * frame_elems;
+        const int64_t lead = (int64_t)(((16u - ((uintptr_t)out & 15u)) & 15u) >> 2);
+        const int64_t head = lead < frame_elems ? lead : frame_elems;
+        const int64_t groups = (frame_elems - head) >> 2;
+        if (tid < head) out[tid] = dequant_u8_fast(src[tid]);
+        const uint8_t* s = src + head;
+        float4* o4 = reinterpret_cast<float4*>(out + head);
+        for (int64_t g = tid; g < groups; g += stride) {
+            const uint8_t* p = s + 4 * g;                               // any alignment: four byte loads
+            o4[g] = make_float4(dequant_u8_fast(p[0]), dequant_u8_fast(p[1]), dequant_u8_fast(p[2]),
+                                dequant_u8_fast(p[3]));
+        }
+        const int64_t tail = head + 4 * groups;
+        if (tid < frame_elems - tail) out[tail + tid] = dequant_u8_fast(s[4 * groups + tid]);
+    }
+}
+
+int decode_warps(int max_row_bytes, int* warps) {
+    USDU_REQUIRE(max_row_bytes >= 1 && max_row_bytes <= USDU_PNG_MAX_ROW_BYTES,
+                 "usdu_png_decode_u8: row bytes %d outside [1, %d]", max_row_bytes, USDU_PNG_MAX_ROW_BYTES);
+    int dev = 0, optin = 0;
+    USDU_CUDA(cudaGetDevice(&dev));
+    USDU_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+    cudaFuncAttributes a;
+    USDU_CUDA(cudaFuncGetAttributes(&a, (const void*)png_decode_kernel));
+    const int64_t fit = ((int64_t)optin - (int64_t)a.sharedSizeBytes) / max_row_bytes;
+    USDU_REQUIRE(fit >= kDecMinWarps, "usdu_png_decode_u8: %d-byte rows leave room for %lld ring rows (need %d)",
+                 max_row_bytes, (long long)fit, kDecMinWarps);
+    *warps = fit < kDecWarps ? (int)fit : kDecWarps;
+    return USDU_OK;
+}
+
 }  // namespace
 }  // namespace usdu
 
@@ -151,18 +198,53 @@ using namespace usdu;
 
 extern "C" {
 
+int usdu_png_decode_warps(int max_row_bytes) {
+    int warps = 0;
+    const int r = decode_warps(max_row_bytes, &warps);
+    return r != USDU_OK ? r : warps;
+}
+
 int usdu_png_decode_u8(const uint8_t* src_dev, const int64_t* segs_dev, int64_t n_segs, const int64_t* descs_dev,
                        int n, int max_row_bytes, uint8_t* dst_dev, void* stream) {
     USDU_REQUIRE(n >= 0, "usdu_png_decode_u8: %d frames", n);
     if (n == 0) return USDU_OK;
     USDU_REQUIRE(src_dev && segs_dev && descs_dev && dst_dev, "usdu_png_decode_u8: null pointer");
     USDU_REQUIRE(n_segs >= 1, "usdu_png_decode_u8: no segments");
-    USDU_REQUIRE(max_row_bytes >= 1 && max_row_bytes <= USDU_PNG_MAX_ROW_BYTES,
-                 "usdu_png_decode_u8: row bytes %d outside [1, %d]", max_row_bytes, USDU_PNG_MAX_ROW_BYTES);
-    const size_t smem = (size_t)kDecWarps * (size_t)max_row_bytes;
-    int r = raise_smem_limit((const void*)png_decode_kernel, smem);
+    int warps = 0;
+    int r = decode_warps(max_row_bytes, &warps);
     if (r != USDU_OK) return r;
-    png_decode_kernel<<<n, kDecThreads, smem, (cudaStream_t)stream>>>(src_dev, segs_dev, n_segs, descs_dev, dst_dev);
+    const size_t smem = (size_t)warps * (size_t)max_row_bytes;
+    r = raise_smem_limit((const void*)png_decode_kernel, smem);
+    if (r != USDU_OK) return r;
+    png_decode_kernel<<<n, warps * 32, smem, (cudaStream_t)stream>>>(src_dev, segs_dev, n_segs, descs_dev, dst_dev);
+    USDU_CUDA(cudaGetLastError());
+    return USDU_OK;
+}
+
+int usdu_gather_unpack_f32(const uint8_t* const* frames_dev, int n, int64_t frame_elems, float* dst, void* stream) {
+    USDU_REQUIRE(n >= 0 && frame_elems >= 0, "usdu_gather_unpack_f32: %d frames of %lld elements", n,
+                 (long long)frame_elems);
+    if (n == 0 || frame_elems == 0) return USDU_OK;
+    USDU_REQUIRE(frames_dev && dst, "usdu_gather_unpack_f32: null pointer");
+    USDU_REQUIRE(((uintptr_t)dst & 3) == 0, "usdu_gather_unpack_f32: dst must be 4-byte aligned");
+    // pinned host memory is written through its device alias (the same address under UVA, cudaHostAlloc)
+    cudaPointerAttributes pa;
+    USDU_CUDA(cudaPointerGetAttributes(&pa, dst));
+    float* out = dst;
+    if (pa.type == cudaMemoryTypeHost) {
+        void* alias = nullptr;
+        USDU_CUDA(cudaHostGetDevicePointer(&alias, dst, 0));
+        out = static_cast<float*>(alias);
+    } else {
+        USDU_REQUIRE(pa.type == cudaMemoryTypeDevice || pa.type == cudaMemoryTypeManaged,
+                     "usdu_gather_unpack_f32: dst is neither device nor pinned host memory");
+    }
+    const int64_t groups = frame_elems / 4 + 1;
+    const int gy = min(n, 65535);
+    const int want = max(1, 4 * grid_sms() / gy);                       // about 4 CTAs per SM over the whole grid
+    const int64_t need = (groups + kThreads - 1) / kThreads;
+    const int gx = need < want ? (int)need : want;
+    gather_unpack_kernel<<<dim3(gx, gy), kThreads, 0, (cudaStream_t)stream>>>(frames_dev, n, frame_elems, out);
     USDU_CUDA(cudaGetLastError());
     return USDU_OK;
 }

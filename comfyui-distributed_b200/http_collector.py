@@ -1,0 +1,473 @@
+"""Master side of the reference's collector transport: its job_complete and prepare_job routes
+(api/job_routes.py:142-157, 273-343) and the master role of DistributedCollector (nodes/collector.py:238-469), with the
+workers' images decoded and assembled on this GPU.
+
+The routes and the job state (multi_job_id -> asyncio.Queue, plus a lock) live on ComfyUI's server event loop, as in
+the reference; the master's prompt thread reaches them with `run_coroutine_threadsafe`.  The job_complete handler checks
+a POST in the reference's order and answers with its status codes and JSON bodies, but never decodes pixels: the base64
+text is decoded on the host with the reference's own call (`b64decode(validate=True)` fixes which texts are accepted),
+and the PNG is validated with http_master.parse_png, which keeps the bytes and the segment table of the filtered rows.
+The master uploads each drained batch of frames and decodes it on a side stream (http_master.PngDecoder) while it waits
+for more, and assembles the result with one usdu_gather_unpack_f32 launch that writes every worker frame, as k / 255,
+straight into the pinned host result in its final order.
+
+Differences from the reference (INTEGRATION.md, "A master for HTTP workers"):
+* images PIL would open but parse_png refuses answer the reference's decode-failure response (500, "Failed to decode
+  PNG image payload: ..."): palette, 16-bit and interlaced PNGs, PNGs with rows over PNG_MAX_ROW_BYTES (16,384 RGBA
+  pixels), and other formats PIL detects (JPEG, BMP, ...).  Neither worker sends any of them;
+* no busy-probe of missing workers (collector.py:374-411 reads the orchestrator's gpu_config.json), and the worker
+  timeout is COMFYUI_HEARTBEAT_TIMEOUT (default 60 s), not the config file's setting;
+* delegate-only mode comes from the node's hidden input only, not from the config file;
+* load_balance is not implemented (the orchestrator's concern), as for the USDU master.
+"""
+from __future__ import annotations
+
+import asyncio
+import base64
+import binascii
+import os
+import time
+import warnings
+from typing import Callable, Dict, List, Optional, Sequence, Tuple
+
+import numpy as np
+
+from .http_master import PngInfo, heartbeat_interval, heartbeat_timeout, parse_png
+
+JOB_INIT_GRACE_PERIOD = 10.0        # utils/constants.py:37: how long a POST waits for its job's queue
+GRACE_POLL = 0.05                   # job_routes.py:333
+EMPTY_AUDIO_SAMPLE_RATE = 44100
+
+
+def max_audio_payload_bytes() -> int:
+    return int(os.environ.get("COMFYUI_MAX_AUDIO_PAYLOAD_BYTES", str(256 * 1024 * 1024)))
+
+
+# --------------------------------------------------------------------------------------
+# request checks (job_routes.py:104-139, utils/audio_payload.py), messages as the reference's
+# --------------------------------------------------------------------------------------
+def field_errors(data: dict) -> List[str]:
+    job_id, worker_id, batch_idx = data.get("job_id"), data.get("worker_id"), data.get("batch_idx")
+    image, audio, is_last = data.get("image"), data.get("audio"), data.get("is_last")
+    errors = []
+    if not isinstance(job_id, str) or not job_id.strip():
+        errors.append("job_id: expected non-empty string")
+    if not isinstance(worker_id, str) or not worker_id.strip():
+        errors.append("worker_id: expected non-empty string")
+    if not isinstance(batch_idx, int) or batch_idx < 0:        # a bool is an int here, as in the reference
+        errors.append("batch_idx: expected non-negative integer")
+    if not isinstance(image, str) or not image.strip():
+        errors.append("image: expected non-empty base64 PNG string")
+    if audio is not None and not isinstance(audio, dict):
+        errors.append("audio: expected object when provided")
+    if not isinstance(is_last, bool):
+        errors.append("is_last: expected boolean")
+    return errors
+
+
+def png_of_payload(image: str) -> Tuple[bytes, PngInfo]:
+    """The image field -> (PNG bytes, their validation), or ValueError with the reference's message."""
+    text = image.strip()
+    if text.startswith("data:"):
+        header, sep, body = text.partition(",")
+        if not sep:
+            raise ValueError("Field 'image' data URL is malformed.")
+        if not header.lower().startswith("data:image/png;base64"):
+            raise ValueError("Field 'image' must be a PNG data URL when using data:* format.")
+        text = body
+    try:
+        png = base64.b64decode(text, validate=True)
+    except (binascii.Error, ValueError) as exc:
+        raise ValueError("Field 'image' is not valid base64 PNG data.") from exc
+    if not png:
+        raise ValueError("Field 'image' decoded to empty PNG data.")
+    try:
+        info = parse_png(png)
+    except Exception as exc:
+        raise ValueError(f"Failed to decode PNG image payload: {exc}") from exc
+    return png, info
+
+
+def audio_of_payload(payload) -> Optional[dict]:
+    """The audio envelope -> AUDIO dict (CPU float32 waveform [batch, channels, samples]), with the reference's rules
+    and messages."""
+    import torch
+    if payload is None:
+        return None
+    if not isinstance(payload, dict):
+        raise ValueError("Field 'audio' must be an object when provided.")
+    text, shape = payload.get("data"), payload.get("shape")
+    rate, dtype = payload.get("sample_rate", 44100), payload.get("dtype", "float32")
+    if not isinstance(text, str) or not text.strip():
+        raise ValueError("Field 'audio.data' must be a non-empty base64 string.")
+    if not isinstance(shape, list) or len(shape) != 3:
+        raise ValueError("Field 'audio.shape' must be a 3-item list [batch, channels, samples].")
+    if dtype != "float32":
+        raise ValueError("Field 'audio.dtype' must be 'float32'.")
+    try:
+        dims = tuple(int(d) for d in shape)
+    except (TypeError, ValueError) as exc:
+        raise ValueError("Field 'audio.shape' must contain integers.") from exc
+    if dims[0] <= 0 or dims[1] <= 0 or dims[2] < 0:
+        raise ValueError("Field 'audio.shape' must be [batch>0, channels>0, samples>=0].")
+    try:
+        rate = int(rate)
+    except (TypeError, ValueError) as exc:
+        raise ValueError("Field 'audio.sample_rate' must be an integer.") from exc
+    if rate <= 0:
+        raise ValueError("Field 'audio.sample_rate' must be positive.")
+    try:
+        raw = base64.b64decode(text, validate=True)
+    except (binascii.Error, ValueError) as exc:
+        raise ValueError("Field 'audio.data' is not valid base64.") from exc
+    limit = max_audio_payload_bytes()
+    if len(raw) > limit:
+        raise ValueError(f"Field 'audio.data' too large: {len(raw)} bytes exceeds {limit}.")
+    want = int(np.prod(dims, dtype=np.int64)) * 4
+    if len(raw) != want:
+        raise ValueError(f"Field 'audio.data' byte size mismatch: expected {want}, got {len(raw)}.")
+    wave = torch.from_numpy(np.frombuffer(raw, dtype=np.float32).reshape(dims).copy())
+    return {"waveform": wave.contiguous(), "sample_rate": rate}
+
+
+# --------------------------------------------------------------------------------------
+# job state: multi_job_id -> queue of received frames, on the server loop
+# --------------------------------------------------------------------------------------
+class CollectorStore:
+    """The collector jobs of one server, touched only on its event loop.  A queue item is {"png", "info",
+    "worker_id", "image_index", "is_last", "audio"}: the PNG as posted (validated, not decoded)."""
+
+    def __init__(self):
+        self.jobs: Dict[str, asyncio.Queue] = {}
+        self._lock: Optional[asyncio.Lock] = None
+
+    @property
+    def lock(self) -> asyncio.Lock:
+        if self._lock is None:
+            self._lock = asyncio.Lock()
+        return self._lock
+
+    async def prepare(self, multi_job_id):
+        async with self.lock:
+            if multi_job_id not in self.jobs:
+                self.jobs[multi_job_id] = asyncio.Queue()
+
+    async def put(self, multi_job_id, item: dict) -> bool:
+        async with self.lock:
+            q = self.jobs.get(multi_job_id)
+            if q is None:
+                return False
+            q.put_nowait(item)
+            return True
+
+    async def take(self, multi_job_id, timeout: float) -> List[dict]:
+        """Wait up to `timeout` for an item, then take it and every item already queued behind it ([] on a time-out
+        or when the job is gone)."""
+        async with self.lock:
+            q = self.jobs.get(multi_job_id)
+        if q is None:
+            return []
+        try:
+            first = await asyncio.wait_for(q.get(), timeout=timeout)
+        except asyncio.TimeoutError:
+            return []
+        return [first] + await self.drain(multi_job_id)
+
+    async def drain(self, multi_job_id) -> List[dict]:
+        async with self.lock:
+            q = self.jobs.get(multi_job_id)
+            out = []
+            while q is not None:
+                try:
+                    out.append(q.get_nowait())
+                except asyncio.QueueEmpty:
+                    break
+            return out
+
+    async def remove(self, multi_job_id):
+        async with self.lock:
+            self.jobs.pop(multi_job_id, None)
+
+
+# --------------------------------------------------------------------------------------
+# routes
+# --------------------------------------------------------------------------------------
+def _error(error, status=500):
+    from aiohttp import web
+    if isinstance(error, list):
+        return web.json_response({"errors": [str(e) for e in error]}, status=status)
+    return web.json_response({"error": str(error)}, status=status)
+
+
+def make_handlers(store: CollectorStore, clock: Callable[[], float] = time.monotonic):
+    """The two route handlers over `store` -> {(method, path): handler}."""
+    from aiohttp import web
+
+    async def prepare_job(request):
+        try:
+            data = await request.json()
+            multi_job_id = data.get("multi_job_id")
+            if not multi_job_id:
+                return _error("Missing multi_job_id", 400)
+            await store.prepare(multi_job_id)
+            return web.json_response({"status": "success"})
+        except Exception as e:
+            return _error(e)
+
+    async def job_complete(request):
+        try:
+            data = await request.json()
+        except Exception as exc:
+            return _error(f"Invalid JSON payload: {exc}", 400)
+        if not isinstance(data, dict):
+            return _error("Expected a JSON object body", 400)
+        try:
+            errors = field_errors(data)
+            if errors:
+                return _error(errors, 400)
+            png, info = png_of_payload(data["image"])
+            audio = audio_of_payload(data.get("audio")) if data.get("audio") is not None else None
+            item = {"png": png, "info": info, "worker_id": data["worker_id"].strip(),
+                    "image_index": int(data["batch_idx"]), "is_last": data["is_last"], "audio": audio}
+            job_id = data["job_id"].strip()
+            deadline = clock() + float(JOB_INIT_GRACE_PERIOD)
+            while not await store.put(job_id, item):
+                if clock() > deadline:
+                    return _error("job not initialized", 404)
+                await asyncio.sleep(GRACE_POLL)
+            return web.json_response({"status": "success"})
+        except Exception as e:
+            return _error(e)
+
+    return {("POST", "/distributed/prepare_job"): prepare_job, ("POST", "/distributed/job_complete"): job_complete}
+
+
+COLLECTOR_ROUTES = (("POST", "/distributed/prepare_job"), ("POST", "/distributed/job_complete"))
+
+STORE = CollectorStore()
+_served: set = set()
+_loop = None
+_warned: set = set()
+
+
+def register(routes, store: CollectorStore = STORE, loop=None) -> set:
+    """Add the handlers to an aiohttp RouteTableDef (ComfyUI's PromptServer.instance.routes), skipping, with one warning
+    each, every path another package already serves.  -> the (method, path) pairs this module serves."""
+    global _loop
+    taken = {(getattr(r, "method", None), getattr(r, "path", None)) for r in routes}
+    served = set()
+    for (method, path), fn in make_handlers(store).items():
+        if (method, path) in taken:
+            if (method, path) not in _warned:
+                _warned.add((method, path))
+                warnings.warn(f"comfyui-distributed_b200: {method} {path} is already served by another package; "
+                              "this package's collector master role stays off", RuntimeWarning, stacklevel=2)
+            continue
+        routes.route(method, path)(fn)
+        served.add((method, path))
+    if store is STORE:
+        _served.update(served)
+        _loop = loop
+    return served
+
+
+def install(routes, loop=None):
+    """Register on ComfyUI's route table once (http_master.install_in_comfyui)."""
+    if not _served:
+        register(routes, STORE, loop)
+
+
+def serving() -> bool:
+    """This process serves the collector routes (and has the server loop to reach them)."""
+    return all(r in _served for r in COLLECTOR_ROUTES) and _server_loop() is not None
+
+
+def _server_loop():
+    if _loop is not None:
+        return _loop
+    try:
+        import server
+        return server.PromptServer.instance.loop
+    except Exception:
+        return None
+
+
+def reset_for_tests():
+    """Forget the registration (test harnesses that start and stop their own server)."""
+    global _loop
+    _served.clear()
+    _loop = None
+    STORE.jobs.clear()
+    STORE._lock = None
+
+
+# --------------------------------------------------------------------------------------
+# frames on the device: decode as they arrive, one gather-unpack into the result
+# --------------------------------------------------------------------------------------
+class GpuFrames:
+    """Each `add`ed batch of queue items is decoded on the side stream into one fresh device buffer, a 16-byte
+    aligned u8 [H, W, 3] slot per frame (item["frame"] = (buffer, offset)).  `assemble` writes the result."""
+
+    def __init__(self, device):
+        from .http_master import PngDecoder
+        self.device = device
+        self.decoder = PngDecoder(device)
+        self.stats = {"upload_ms": 0.0, "decode_ms": 0.0, "assembly_ms": 0.0, "decode_launches": 0}
+
+    def add(self, items: Sequence[dict]):
+        import torch
+        if not items:
+            return
+        offs, cur = [], 0
+        for it in items:
+            offs.append(cur)
+            cur += (it["info"].H * it["info"].W * 3 + 15) // 16 * 16
+        with torch.cuda.device(self.device):
+            buf = torch.empty(max(cur, 16), dtype=torch.uint8, device=self.device)
+        self.decoder.decode([(it["info"], it["png"], o) for it, o in zip(items, offs)], buf)
+        for it, o in zip(items, offs):
+            it["frame"] = (buf, o)
+        self.stats["decode_launches"] += 1
+
+    def assemble(self, head, items: Sequence[dict], shape: Tuple[int, int, int], dtype):
+        """-> CPU tensor [len(head) + len(items), *shape] of `dtype`: `head` (the master's frames, any device, or None)
+        converted to dtype, then each item's frame as k / 255 in float32 (then dtype).  Pinned memory; the worker
+        frames go through usdu_gather_unpack_f32 straight into it (or into a float32 pinned buffer when dtype is not
+        float32)."""
+        import torch
+        from . import _native as nat
+        M = 0 if head is None else int(head.shape[0])
+        n = len(items)
+        H, W, C = shape
+        out = torch.empty((M + n, H, W, C), dtype=dtype, pin_memory=True)
+        with torch.cuda.device(self.device):
+            main = torch.cuda.current_stream()
+            main.wait_stream(self.decoder.side)
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            if M:
+                out[:M].copy_(head, non_blocking=head.is_cuda)
+            if n:
+                dst = out[M:] if dtype == torch.float32 else torch.empty((n, H, W, C), dtype=torch.float32,
+                                                                          pin_memory=True)
+                ptrs = torch.tensor([buf.data_ptr() + o for buf, o in (it["frame"] for it in items)], dtype=torch.int64)
+                ptrs = ptrs.to(self.device, non_blocking=False)
+                nat.gather_unpack_f32(ptrs.data_ptr(), n, H * W * C, dst.data_ptr(), main.cuda_stream)
+            e1.record()
+            main.synchronize()
+            if n and dtype != torch.float32:
+                out[M:].copy_(dst)
+        self.stats["assembly_ms"] = e0.elapsed_time(e1)
+        self.stats["upload_ms"], self.stats["decode_ms"] = self.decoder.times()
+        self.decoder.release()
+        return out
+
+
+# --------------------------------------------------------------------------------------
+# the master role (nodes/collector.py:238-469)
+# --------------------------------------------------------------------------------------
+class HttpCollectorMaster:
+    """One collector job with this process as the master of HTTP workers.  `frames` decodes and assembles (GpuFrames
+    on the master's device unless given)."""
+
+    def __init__(self, multi_job_id: str, enabled_workers: Sequence, store: CollectorStore = STORE, loop=None,
+                 frames=None, device=None):
+        self.multi_job_id = multi_job_id
+        self.workers: List[str] = []
+        for w in enabled_workers:                       # de-duplicated, in order (collector.py:247-255)
+            if str(w) not in self.workers:
+                self.workers.append(str(w))
+        self.store, self.loop = store, loop if loop is not None else _server_loop()
+        if self.loop is None:
+            raise RuntimeError("HttpCollectorMaster: no server event loop")
+        self.frames, self.device = frames, device
+        self.stats: dict = {"bytes_received": 0}
+
+    def _call(self, coro, timeout: Optional[float] = 10.0):
+        return asyncio.run_coroutine_threadsafe(coro, self.loop).result(timeout)
+
+    def run(self, images, audio=None, delegate_only: bool = False):
+        """-> (images, audio) as the reference's master returns them."""
+        import torch
+        from .nodes.collector import combine_audio
+        empty = {"waveform": torch.zeros(1, 2, 1), "sample_rate": EMPTY_AUDIO_SAMPLE_RATE}
+        job = self.multi_job_id
+        self._call(self.store.prepare(job))             # the queue exists before any local work (collector.py:261-268)
+        try:
+            if self.frames is None:
+                dev = images.device if images.is_cuda else torch.device("cuda", torch.cuda.current_device())
+                self.frames = GpuFrames(self.device if self.device is not None else dev)
+            held, worker_audio = self._collect()
+        finally:
+            self._call(self.store.remove(job))
+        head = None if delegate_only or images.shape[0] == 0 else images
+        order = self.workers + sorted(w for w in held if w not in self.workers)
+        items = [held[w][i] for w in order if w in held for i in sorted(held[w])]
+        audios = [None if delegate_only else audio] + [worker_audio.get(w) for w in self.workers] + \
+                 [worker_audio[w] for w in sorted(worker_audio) if w not in self.workers]
+        self.stats.update(order=[w for w in order if w in held], frames={w: len(held[w]) for w in order if w in held})
+        if not items:                                   # the master's frames alone, or the reference's fallback_images
+            out = images.contiguous() if head is None else images.cpu().clone(memory_format=torch.contiguous_format)
+            return out, combine_audio(audios, empty)
+        shapes = {(it["info"].H, it["info"].W, 3) for it in items}
+        if head is not None:
+            shapes.add(tuple(int(v) for v in images.shape[1:]))
+        if len(shapes) != 1:
+            # torch.cat would fail: the reference's except returns the master's own images and audio
+            self.stats["fallback"] = f"frames of different shapes: {sorted(shapes)}"
+            return images, audio if audio is not None else empty
+        dtype = torch.float32 if head is None else torch.promote_types(images.dtype, torch.float32)
+        out = self.frames.assemble(head, items, shapes.pop(), dtype)
+        self.stats.update(self.frames.stats)
+        return out, combine_audio(audios, empty)
+
+    def _collect(self):
+        """collector.py:289-446: -> ({worker: {image_index: item}}, {worker: last audio})."""
+        mm = _comfy_mm()
+        job = self.multi_job_id
+        expected, done = set(self.workers), set()
+        held: Dict[str, Dict[int, dict]] = {}
+        worker_audio: Dict[str, dict] = {}
+        timeout = heartbeat_timeout()
+        slice_s = min(max(0.1, heartbeat_interval() / 20.0), timeout)
+        last_activity = time.time()
+
+        def keep(item):
+            held.setdefault(item["worker_id"], {})[item["image_index"]] = item
+            if item["is_last"] and item["worker_id"] in expected:
+                done.add(item["worker_id"])
+
+        while len(done) < len(expected):
+            if mm is not None:
+                mm.throw_exception_if_processing_interrupted()
+            got = self._call(self.store.take(job, slice_s), slice_s + 10.0)
+            self.stats["bytes_received"] += sum(len(it["png"]) for it in got)
+            if got:
+                for item in got:
+                    keep(item)
+                    if item.get("audio") is not None:
+                        worker_audio[item["worker_id"]] = item["audio"]
+                self.frames.add(got)
+                last_activity = time.time()
+                timeout = heartbeat_timeout()
+                continue
+            if time.time() - last_activity < timeout:
+                continue
+            if mm is not None:
+                mm.throw_exception_if_processing_interrupted()
+            # the workers still missing timed out: take what is queued (its audio is not kept, collector.py:419-437)
+            rest = self._call(self.store.drain(job))
+            self.stats["bytes_received"] += sum(len(it["png"]) for it in rest)
+            for item in rest:
+                keep(item)
+            self.frames.add(rest)
+            break
+        return held, worker_audio
+
+
+def _comfy_mm():
+    try:
+        import comfy.model_management as mm
+        return mm
+    except ImportError:
+        return None

@@ -30,6 +30,8 @@ from typing import Callable, Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 
+from ._native import PNG_MAX_ROW_BYTES
+
 PNG_SIGNATURE = b"\x89PNG\r\n\x1a\n"
 CHANNELS = {0: 1, 2: 3, 4: 2, 6: 4}          # PNG colour type -> samples per pixel (8-bit)
 REQUEST_WAIT = 0.1                            # request_image's wait on an empty queue (usdu_routes.py:195)
@@ -71,7 +73,7 @@ def parse_png(data: bytes) -> PngInfo:
     reason otherwise.  Checks: signature; IHDR (8-bit, colour type 0/2/4/6, no interlace); chunk bounds; the CRC-32 of
     every chunk before the first IDAT (PIL checks those, not IDAT's or later ones); the zlib header; the stored-block
     LEN/NLEN chain (any compressed block: the stream is inflated with zlib); the Adler-32; the IDAT length against the
-    image size; every filter byte <= 4."""
+    image size; every filter byte <= 4; rows of at most PNG_MAX_ROW_BYTES (what the decode kernel takes)."""
     mv = memoryview(data)
     n = len(data)
     if n < 8 or data[:8] != PNG_SIGNATURE:
@@ -105,6 +107,8 @@ def parse_png(data: bytes) -> PngInfo:
                 raise ValueError("unknown compression or filter method")
             if interlace != 0:
                 raise ValueError("unsupported PNG: interlaced")
+            if W * CHANNELS[color] > PNG_MAX_ROW_BYTES:
+                raise ValueError(f"unsupported PNG: rows of {W * CHANNELS[color]} bytes (at most {PNG_MAX_ROW_BYTES})")
             ihdr = (W, H, CHANNELS[color])
         elif ctype == b"IDAT":
             if idat and idat[-1][0] + idat[-1][1] + 4 != pos:
@@ -602,15 +606,19 @@ def register(routes, store: JobStore = STORE, loop=None) -> set:
 
 
 def install_in_comfyui():
-    """Register the routes on server.PromptServer.instance when imported inside ComfyUI; a no-op elsewhere."""
+    """Register the routes of this module and of http_collector on server.PromptServer.instance when imported inside
+    ComfyUI; a no-op elsewhere."""
     try:
         import server
         inst = server.PromptServer.instance
     except Exception:
         return
-    if inst is None or getattr(inst, "routes", None) is None or _served:
+    if inst is None or getattr(inst, "routes", None) is None:
         return
-    register(inst.routes, STORE, getattr(inst, "loop", None))
+    if not _served:
+        register(inst.routes, STORE, getattr(inst, "loop", None))
+    from . import http_collector
+    http_collector.install(inst.routes, getattr(inst, "loop", None))
 
 
 def serving() -> bool:
@@ -638,6 +646,67 @@ def reset_for_tests():
 
 
 # --------------------------------------------------------------------------------------
+# decode on the device as frames arrive (csrc/usdu_png_decode.cu)
+# --------------------------------------------------------------------------------------
+class PngDecoder:
+    """Uploads batches of validated PNGs through pinned memory and decodes each batch with one usdu_png_decode_u8
+    launch on a side stream, so the caller can go on waiting for more.  A batch's staging stays alive until
+    `release()`; `times()` (after the side stream has finished) sums the upload and decode times of every batch."""
+
+    def __init__(self, device):
+        import torch
+        self.device = device
+        with torch.cuda.device(device):
+            self.side = torch.cuda.Stream(device)
+        self._events = []
+        self._keep_alive = []
+
+    def decode(self, items: Sequence[Tuple[PngInfo, bytes, int]], dst):
+        """items: (info, PNG bytes, byte offset of the frame's [H, W, 3] u8 output in the device tensor `dst`)."""
+        import torch
+        from . import _native as nat
+        if not items:
+            return
+        blobs, segs, descs, pos, max_row = [], [], [], 0, 1
+        for info, png, off in items:
+            blob = info.inflated if info.inflated is not None else png
+            descs.append([len(segs), len(info.segs), info.H, info.W, info.C, off, 0, 0])
+            segs.extend((pos + o, r) for o, r in info.segs)
+            blobs.append(blob)
+            pos += len(blob)
+            max_row = max(max_row, info.W * info.C)
+        tabs = np.concatenate([np.asarray(segs, np.int64).reshape(-1), np.asarray(descs, np.int64).reshape(-1)])
+        nbytes = (pos + 15) // 16 * 16 + tabs.nbytes
+        host = torch.empty(nbytes, dtype=torch.uint8, pin_memory=True)
+        h = host.numpy()
+        o = 0
+        for blob in blobs:
+            h[o: o + len(blob)] = np.frombuffer(blob, np.uint8)
+            o += len(blob)
+        t0 = (pos + 15) // 16 * 16
+        h[t0:] = tabs.view(np.uint8)
+        with torch.cuda.device(self.device), torch.cuda.stream(self.side):
+            dev = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+            e_up, e0, e1 = (torch.cuda.Event(enable_timing=True) for _ in range(3))
+            e_up.record(self.side)
+            dev.copy_(host, non_blocking=True)
+            e0.record(self.side)
+            nat.png_decode_u8(dev.data_ptr(), dev.data_ptr() + t0, len(segs), dev.data_ptr() + t0 + 16 * len(segs),
+                              len(descs), max_row, dst.data_ptr(), self.side.cuda_stream)
+            e1.record(self.side)
+        self._events.append((e_up, e0, e1))
+        self._keep_alive.append((host, dev, dst))
+
+    def times(self) -> Tuple[float, float]:
+        """-> (upload ms, decode ms) over every batch so far; the side stream must have finished."""
+        return (sum(a.elapsed_time(b) for a, b, _ in self._events),
+                sum(b.elapsed_time(c) for _, b, c in self._events))
+
+    def release(self):
+        self._keep_alive.clear()
+
+
+# --------------------------------------------------------------------------------------
 # the master role (static.py:371-570) on the device
 # --------------------------------------------------------------------------------------
 class HttpStaticMaster:
@@ -662,13 +731,11 @@ class HttpStaticMaster:
         self.device = job.device
         with torch.cuda.device(self.device):
             self.payload = torch.empty(max(cur, 16), dtype=torch.uint8, device=self.device)
-            self.side = torch.cuda.Stream(self.device)
+        self.decoder = PngDecoder(self.device)
         self.master_ids: List[int] = []
         self.kept: Dict[str, List[int]] = {}
         self.stats = {"bytes_received": 0, "tiles_received": 0, "upload_ms": 0.0, "decode_ms": 0.0,
                       "decode_launches": 0, "blend_ms": 0.0}
-        self._decode_events = []
-        self._keep_alive = []
 
     # -- event-loop calls ---------------------------------------------------------------
     def _call(self, coro, timeout: Optional[float] = 5.0):
@@ -684,9 +751,7 @@ class HttpStaticMaster:
     # -- decode as results arrive ---------------------------------------------------------
     def _decode(self, entries: List[Tuple[int, dict]]):
         """Upload the PNG bytes of `entries` through pinned memory and decode them on the side stream."""
-        import torch
-        from . import _native as nat
-        todo = []
+        items = []
         for g, e in entries:
             b = e.get("batch_idx", g // self.T)
             t = e["tile_idx"]
@@ -695,42 +760,13 @@ class HttpStaticMaster:
             self.kept.setdefault(str(e["worker_id"]), [])
             if t not in self.kept[str(e["worker_id"])]:
                 self.kept[str(e["worker_id"])].append(t)
-            todo.append((t, b, e))
-        if not todo:
-            return
-        blobs, segs, descs, pos, max_row = [], [], [], 0, 1
-        for t, b, e in todo:
             info = e["info"]
-            blob = info.inflated if info.inflated is not None else e["png"]
-            descs.append([len(segs), len(info.segs), info.H, info.W, info.C,
-                          self.base[t] + b * info.H * info.W * 3, 0, 0])
-            segs.extend((pos + o, r) for o, r in info.segs)
-            blobs.append(blob)
-            pos += len(blob)
-            max_row = max(max_row, info.W * info.C)
+            items.append((info, e["png"], self.base[t] + b * info.H * info.W * 3))
             self.stats["bytes_received"] += len(e["png"])
-        self.stats["tiles_received"] += len(todo)
-        tabs = np.concatenate([np.asarray(segs, np.int64).reshape(-1), np.asarray(descs, np.int64).reshape(-1)])
-        nbytes = (pos + 15) // 16 * 16 + tabs.nbytes
-        host = torch.empty(nbytes, dtype=torch.uint8, pin_memory=True)
-        h = host.numpy()
-        o = 0
-        for blob in blobs:
-            h[o: o + len(blob)] = np.frombuffer(blob, np.uint8)
-            o += len(blob)
-        t0 = (pos + 15) // 16 * 16
-        h[t0:] = tabs.view(np.uint8)
-        with torch.cuda.device(self.device), torch.cuda.stream(self.side):
-            dev = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
-            e_up, e0, e1 = (torch.cuda.Event(enable_timing=True) for _ in range(3))
-            e_up.record(self.side)
-            dev.copy_(host, non_blocking=True)
-            e0.record(self.side)
-            nat.png_decode_u8(dev.data_ptr(), dev.data_ptr() + t0, len(segs), dev.data_ptr() + t0 + 16 * len(segs),
-                              len(descs), max_row, self.payload.data_ptr(), self.side.cuda_stream)
-            e1.record(self.side)
-        self._decode_events.append((e_up, e0, e1))
-        self._keep_alive.append((host, dev))
+        if not items:
+            return
+        self.stats["tiles_received"] += len(items)
+        self.decoder.decode(items, self.payload)
         self.stats["decode_launches"] += 1
 
     # -- the job --------------------------------------------------------------------------
@@ -808,7 +844,7 @@ class HttpStaticMaster:
         canvas = self.job.canvas
         with torch.cuda.device(self.device):
             main = torch.cuda.current_stream()
-            main.wait_stream(self.side)
+            main.wait_stream(self.decoder.side)
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
             tiles = sorted(have)
@@ -827,9 +863,8 @@ class HttpStaticMaster:
             out = canvas.result()
             main.synchronize()
         self.stats["blend_ms"] = e0.elapsed_time(e1)
-        self.stats["upload_ms"] = sum(a.elapsed_time(b) for a, b, _ in self._decode_events)
-        self.stats["decode_ms"] = sum(b.elapsed_time(c) for _, b, c in self._decode_events)
-        self._keep_alive.clear()
+        self.stats["upload_ms"], self.stats["decode_ms"] = self.decoder.times()
+        self.decoder.release()
         return out
 
     def assignment(self) -> List[List[int]]:

@@ -11,6 +11,11 @@ Started by the reference's orchestrator as an HTTP worker (no torch.distributed 
 the reference's master as that worker does: one job_complete POST per image with a level-0 PNG in base64
 (http_worker.send_collector_batch).  The cast, the PNG layout and the base64 text are computed on the GPU
 (usdu_png_base64_u8); only the finished text goes to the host.
+
+As the master of HTTP workers (no torch.distributed peers, enabled workers, and this process serving the reference's
+job_complete route, http_collector.py), the node collects their images as the reference's master does
+(collector.py:238-469): each worker's PNGs are decoded on the GPU as they arrive, and one launch writes every worker
+frame, as k / 255, into the result after the master's own frames.
 """
 from __future__ import annotations
 
@@ -19,7 +24,7 @@ import json
 import torch
 
 from .. import dist as usdu_dist
-from .. import http_worker
+from .. import http_collector, http_worker
 from ..casts import reference_f32
 
 PNG_TEXT_BUDGET = 64 << 20    # pinned host bytes for one group of frames' base64 text (at least one frame)
@@ -142,6 +147,8 @@ class DistributedCollectorNode:
     # the HTTP worker's cast (IMAGE -> u8 frames) and encoder (u8 frames -> base64 PNG texts)
     pack = staticmethod(_native_pack)
     encode = staticmethod(_native_png_b64)
+    # the HTTP master's decode and assembly (None: http_collector.GpuFrames on the master's device)
+    frames = None
 
     @classmethod
     def INPUT_TYPES(s):
@@ -182,6 +189,13 @@ class DistributedCollectorNode:
             if is_worker:   # an HTTP worker of the reference's orchestrator: send to its master (collector.py:239-243)
                 send_to_master(images, audio, multi_job_id, master_url, worker_id, pack=self.pack, encode=self.encode)
                 return (images, audio if audio is not None else self.EMPTY_AUDIO)
+            if enabled and http_collector.serving():
+                # this process serves job_complete: collect the HTTP workers' images (collector.py:244-469)
+                master = http_collector.HttpCollectorMaster(multi_job_id, enabled, frames=self.frames)
+                try:
+                    return master.run(images, audio, bool(delegate_only))
+                finally:
+                    self.last_stats = master.stats
             return (images, audio if audio is not None else empty_audio)   # no participants (collector.py:255-256)
         wid = worker_id if (worker_id or rank == 0) else f"rank{rank}"
         if not enabled:  # SPMD launch without the reference's orchestrator: every rank is enabled

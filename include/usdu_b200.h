@@ -35,7 +35,7 @@ extern "C" {
 #pragma GCC visibility push(default) /* the library itself is built with -fvisibility=hidden */
 #endif
 
-#define USDU_ABI_VERSION 12
+#define USDU_ABI_VERSION 13
 
 typedef enum usdu_status {
     USDU_OK = 0,
@@ -310,11 +310,22 @@ int usdu_png_base64_u8(const uint8_t* src_dev, int B, int H, int W, int C, uint8
  * descs_dev: n descriptors of USDU_PNG_DESC_WORDS int64: first segment, segment count, H, W, C (1 grey, 2 grey+alpha,
  *   3 RGB, 4 RGBA), byte offset of the frame's [H, W, 3] u8 output in dst_dev, 0, 0.
  * The rows are un-filtered (None / Sub / Up / Avg / Paeth) and converted as PIL's convert("RGB"): grey replicated,
- * alpha dropped.  max_row_bytes >= every frame's W*C and <= USDU_PNG_MAX_ROW_BYTES (shared memory holds 16 rows). */
+ * alpha dropped.  max_row_bytes >= every frame's W*C and <= USDU_PNG_MAX_ROW_BYTES (16,384 px, ComfyUI's
+ * MAX_RESOLUTION, at 4 channels).  Shared memory holds a ring of usdu_png_decode_warps(max_row_bytes) rows, one per
+ * warp of the CTA: min(16, opt-in shared memory per block / max_row_bytes), 3 at the limit on an H100.
+ * usdu_png_decode_warps returns that depth for the current device, or a negative usdu_status. */
 #define USDU_PNG_DESC_WORDS 8
-#define USDU_PNG_MAX_ROW_BYTES 14336
+#define USDU_PNG_MAX_ROW_BYTES 65536
 int usdu_png_decode_u8(const uint8_t* src_dev, const int64_t* segs_dev, int64_t n_segs, const int64_t* descs_dev,
                        int n, int max_row_bytes, uint8_t* dst_dev, void* stream);
+int usdu_png_decode_warps(int max_row_bytes);
+
+/* Collector master's assembly (nodes/collector.py:193-236 after api/job_routes.py:126-130): frame i of n, a u8 frame
+ * of frame_elems bytes at frames_dev[i] (a device array of n device pointers), goes to dst + i * frame_elems as
+ * k / 255.0f, bit-identical to usdu_unpack_tiles_f32.  dst (4-byte aligned) is device memory or pinned host memory
+ * (cudaHostAlloc); the latter is written through its device alias, so one launch performs the conversion and the
+ * device-to-host transfer. */
+int usdu_gather_unpack_f32(const uint8_t* const* frames_dev, int n, int64_t frame_elems, float* dst, void* stream);
 
 /* TEST DOUBLE, not part of the reference path: the deterministic T0 sampler stand-in used by the
  * parity tests and bench.py (BASELINE.md section 3) as one fused pass,
