@@ -16,7 +16,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libusdu_b200.so")
 
 # constants mirrored from include/usdu_b200.h (checked against the header in tests)
-ABI_VERSION = 13
+ABI_VERSION = 14
 ERR_INVALID = -1
 CANVAS_SLACK = 16
 PLAN_INFO_WORDS = 16
@@ -52,7 +52,6 @@ JOB_WORDS = 32
 (J_SRC_A, J_SRC_B, J_LEAD, J_COLS, J_ROWS, J_IX0, J_IY0, J_ROWS_H, J_OX_BASE, J_N_OUT_H, J_ROWS_V, J_OY_BASE, J_N_OUT_V,
  J_DST_X, J_DST_Y, J_OFF_LO, J_OFF_HI, J_ROWS_OUT, J_COLS_OUT, J_CX0, J_CX1, J_CY0, J_CY1, J_FLAGS, J_MPITCH, J_PITCH,
  J_FRAME_LO, J_FRAME_HI, J_NEXT, J_TAPS_H, J_TAPS_V) = range(31)
-J_SLOT = 31
 
 
 class NativeError(RuntimeError):
@@ -79,8 +78,6 @@ _SIGNATURES = {
     "usdu_quantize_canvas": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int64, c_void_p]),
     "usdu_dequantize_canvas": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int64, c_void_p]),
     "usdu_gather_dequantize": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int64, c_void_p]),
-    "usdu_level_blend_crop": (c_int, [c_void_p, c_int, c_int, c_int, c_int64, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int,
-                                      c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p]),
     "usdu_gather_canvas": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int64, c_void_p]),
     "usdu_tile_crop_resize_f32": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p]),
     "usdu_quantize_rows": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int64, c_int, c_int, c_void_p]),
@@ -122,10 +119,9 @@ _SIGNATURES = {
     "usdu_plan_mask_specs": (c_int, [c_void_p, POINTER(c_int32)]),
     "usdu_plan_neighbors": (c_int, [c_void_p, POINTER(c_int32), POINTER(c_int32)]),
     "usdu_plan_waves": (c_int, [c_void_p, POINTER(c_int32), c_int, POINTER(c_int32)]),
-    "usdu_plan_crop_worklist": (c_int, [c_void_p, POINTER(c_int32), c_int, c_int, c_int, c_int, c_int, c_int,
-                                        POINTER(c_void_p)]),
+    "usdu_plan_crop_worklist": (c_int, [c_void_p, POINTER(c_int32), c_int, c_int, c_int, c_int, c_int, POINTER(c_void_p)]),
     "usdu_plan_blend_worklist": (c_int, [c_void_p, POINTER(c_int32), POINTER(c_int64), c_int, c_int, c_int, c_int, c_int,
-                                         c_int, c_int, POINTER(c_int64), c_int, c_int, c_int, c_int, POINTER(c_void_p)]),
+                                         c_int, c_int, c_int, POINTER(c_void_p)]),
     "usdu_worklist_destroy": (c_int, [c_void_p]),
     "usdu_worklist_info": (c_int, [c_void_p, POINTER(c_int64)]),
     "usdu_worklist_items": (c_int, [c_void_p, POINTER(c_int32)]),
@@ -326,11 +322,11 @@ class NativePlan:
         _check(min(st, 0), "usdu_plan_waves")
         return level[:ids.size]
 
-    def crop_worklist(self, tile_ids, B: int, path: int, share: int, sm_count: int, mma_block_rows: int) -> dict:
+    def crop_worklist(self, tile_ids, B: int, path: int, sm_count: int, mma_block_rows: int) -> dict:
         ids = _ids(tile_ids)
         h = c_void_p()
-        _check(self._lib.usdu_plan_crop_worklist(self._h, _i32p(ids), ids.size, B, path, share, sm_count, mma_block_rows,
-                                                 ctypes.byref(h)), "usdu_plan_crop_worklist")
+        _check(self._lib.usdu_plan_crop_worklist(self._h, _i32p(ids), ids.size, B, path, sm_count, mma_block_rows, ctypes.byref(h)),
+               "usdu_plan_crop_worklist")
         slots = np.zeros(max(ids.size, 1), np.int64)
         if ids.size:
             _check(self._lib.usdu_worklist_slots(h, _i64p(slots)), "usdu_worklist_slots")
@@ -338,21 +334,17 @@ class NativePlan:
         out["slots"] = slots[:ids.size]
         return out
 
-    def blend_worklist(self, tile_ids, offs, src_bytes: int, B: int, path: int, part, share: int, rects, keep: int,
-                       sm_count: int, mma_block_rows: int) -> dict:
-        """part = (i, n) or None; rects int64 [m, 4] with keep 1 / 0, or keep = -1 for every block."""
+    def blend_worklist(self, tile_ids, offs, src_bytes: int, B: int, path: int, part, sm_count: int, mma_block_rows: int) -> dict:
+        """part = (i, n) or None."""
         ids = _ids(tile_ids)
         offs = np.ascontiguousarray(np.asarray(offs, dtype=np.int64).reshape(-1))
         if offs.size < ids.size:
             raise ValueError(f"blend work list: {offs.size} source offsets for {ids.size} tiles")
         offs = np.ascontiguousarray(offs[:max(ids.size, 1)]) if offs.size else np.zeros(1, np.int64)
-        rects = np.zeros((0, 4), np.int64) if rects is None else np.asarray(rects, dtype=np.int64).reshape(-1, 4)
-        rbuf = np.ascontiguousarray(rects if rects.size else np.zeros((1, 4), np.int64))
         pi, pn = part if part is not None else (0, 0)
         h = c_void_p()
-        _check(self._lib.usdu_plan_blend_worklist(self._h, _i32p(ids), _i64p(offs), ids.size, src_bytes, B, path, pi, pn, share,
-                                                  _i64p(rbuf), rects.shape[0], keep, sm_count, mma_block_rows, ctypes.byref(h)),
-               "usdu_plan_blend_worklist")
+        _check(self._lib.usdu_plan_blend_worklist(self._h, _i32p(ids), _i64p(offs), ids.size, src_bytes, B, path, pi, pn,
+                                                  sm_count, mma_block_rows, ctypes.byref(h)), "usdu_plan_blend_worklist")
         return _read_worklist(h)
 
 
@@ -407,13 +399,6 @@ def gather_dequantize(slab_ptrs, slab_rows, img_ptr, B, H, W, pitch, stream):
     ptrs = (ctypes.c_void_p * n)(*[int(p) for p in slab_ptrs])
     rows = (c_int32 * (n + 1))(*[int(r) for r in slab_rows])
     _check(lib().usdu_gather_dequantize(ptrs, rows, n, img_ptr, B, H, W, pitch, stream), "usdu_gather_dequantize")
-
-
-def level_blend_crop(canvas_ptr, B, H, W, pitch, tabs_ptr, mask_ptr, bjobs_ptr, n_bheads, b_patch_w, b_patch_h, src_ptr, block_rows,
-                     cjobs_ptr, n_cjobs, c_patch_w, c_patch_h, out_ptr, expect_ptr, n_slots, sync_ptr, flags, stream):
-    _check(lib().usdu_level_blend_crop(canvas_ptr, B, H, W, pitch, tabs_ptr, mask_ptr, bjobs_ptr, n_bheads, b_patch_w, b_patch_h, src_ptr,
-                                       block_rows, cjobs_ptr, n_cjobs, c_patch_w, c_patch_h, out_ptr, expect_ptr, n_slots, sync_ptr,
-                                       flags, stream), "usdu_level_blend_crop")
 
 
 def gather_canvas(slab_ptrs, slab_rows, canvas_ptr, B, H, W, pitch, stream):

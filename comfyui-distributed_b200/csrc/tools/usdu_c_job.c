@@ -181,7 +181,7 @@ int main(int argc, char** argv) {
 
         /* crop: canvas windows -> fp32 tiles at processing size, packed in list order */
         usdu_worklist* cw = NULL;
-        check(usdu_plan_crop_worklist(plan, ids, n, B, 2, 1, 0, 0, &cw), "usdu_plan_crop_worklist");
+        check(usdu_plan_crop_worklist(plan, ids, n, B, 2, 0, 0, &cw), "usdu_plan_crop_worklist");
         int64_t ci[USDU_WL_INFO_WORDS];
         check(usdu_worklist_info(cw, ci), "usdu_worklist_info");
         const size_t citems_bytes = (size_t)(ci[USDU_WL_ITEMS] * ci[USDU_WL_ITEM_WORDS]) * sizeof(int32_t);
@@ -217,7 +217,7 @@ int main(int argc, char** argv) {
 
         /* blend: the sampler output back into the canvas, in list order */
         usdu_worklist* bw = NULL;
-        check(usdu_plan_blend_worklist(plan, ids, slots, n, 4, B, 2, 0, 0, 1, NULL, 0, -1, 0, 0, &bw), "usdu_plan_blend_worklist");
+        check(usdu_plan_blend_worklist(plan, ids, slots, n, 4, B, 2, 0, 0, 0, 0, &bw), "usdu_plan_blend_worklist");
         int64_t bi[USDU_WL_INFO_WORDS];
         check(usdu_worklist_info(bw, bi), "usdu_worklist_info");
         const size_t bitems_bytes = (size_t)(bi[USDU_WL_ITEMS] * bi[USDU_WL_ITEM_WORDS]) * sizeof(int32_t);

@@ -560,10 +560,6 @@ int launch_crop(const void* canvas, int src_f32, int B, int H, int W, int64_t pi
 int launch_blend(uint8_t* canvas, int B, int H, int W, int64_t pitch, const int32_t* tabs, const uint8_t* mask_pool,
                  const int32_t* items, int n_items, int patch_w, int patch_h, const void* src, int src_is_u8, int block_rows,
                  int two_ksteps, cudaStream_t st);
-int launch_level(uint8_t* canvas, int B, int H, int W, int64_t pitch, const int32_t* tabs, const uint8_t* mask_pool,
-                 const int32_t* bjobs, int n_bheads, int b_patch_w, int b_patch_h, const float* src, int block_rows,
-                 const int32_t* cjobs, int n_cjobs, int c_patch_w, int c_patch_h, float* out, const int32_t* expect, int n_slots,
-                 int* sync, int two_ksteps, cudaStream_t st);
 } }
 
 using namespace usdu;
@@ -925,21 +921,6 @@ int usdu_tile_crop_resize_f32(const float* image_dev, int B, int H, int W, const
     if (n_items == 0) return USDU_OK;
     return mma::launch_crop(image_dev, 1, B, H, W, (int64_t)W * 3, tabs_dev, items_dev, n_items, patch_w, patch_h, out_dev,
                             (flags & USDU_FLAG_MMA_KS2) ? 1 : 0, (cudaStream_t)stream);
-}
-
-int usdu_level_blend_crop(uint8_t* canvas_dev, int B, int H, int W, int64_t pitch, const int32_t* tabs_dev,
-                          const uint8_t* mask_pool_dev, const int32_t* bjobs_dev, int n_bheads, int b_patch_w, int b_patch_h,
-                          const float* src_dev, int block_rows, const int32_t* cjobs_dev, int n_cjobs, int c_patch_w, int c_patch_h,
-                          float* out_dev, const int32_t* expect_dev, int n_slots, int32_t* sync_dev, int flags, void* stream) {
-    USDU_REQUIRE(canvas_dev && tabs_dev && mask_pool_dev && bjobs_dev && src_dev && cjobs_dev && out_dev && expect_dev && sync_dev,
-                 "usdu_level_blend_crop: null pointer");
-    USDU_REQUIRE(B > 0 && B <= 65535 && H > 0 && W > 0 && n_bheads > 0 && n_cjobs > 0 && n_slots > 0, "usdu_level_blend_crop: bad shape");
-    USDU_REQUIRE(pitch >= 3LL * W && pitch % 16 == 0, "usdu_level_blend_crop: pitch must be >= 3*W and a multiple of 16");
-    USDU_REQUIRE(((uintptr_t)src_dev & 15) == 0, "usdu_level_blend_crop: src must be 16-byte aligned");
-    USDU_REQUIRE(flags & USDU_FLAG_MMA, "usdu_level_blend_crop: tensor-core job records only (USDU_FLAG_MMA)");
-    return mma::launch_level(canvas_dev, B, H, W, pitch, tabs_dev, mask_pool_dev, bjobs_dev, n_bheads, b_patch_w, b_patch_h, src_dev,
-                             block_rows, cjobs_dev, n_cjobs, c_patch_w, c_patch_h, out_dev, expect_dev, n_slots, sync_dev,
-                             (flags & USDU_FLAG_MMA_KS2) ? 1 : 0, (cudaStream_t)stream);
 }
 
 int usdu_tile_blend(uint8_t* canvas_dev, int B, int H, int W, int64_t pitch, const int32_t* tiles_dev,

@@ -575,176 +575,6 @@ blend_mma_kernel(const int32_t* __restrict__ tabs, const uint8_t* __restrict__ m
     }
 }
 
-// ======================================================================================
-// one launch per dependency level: blend of wave k  U  crop of wave k + 1
-// ======================================================================================
-// The progressive job is a chain  crop(k) -> sampler(k) -> blend(k) -> crop(k+1) -> ...  (upscale/modes/single_gpu.py:
-// 40-64).  blend(k) and crop(k+1) have no sampler between them, and a crop of wave k+1 needs only the one or two tiles of
-// wave k whose windows touch its own.  This kernel runs both in ONE grid: work items are taken from an atomic ticket
-// (all blend items first, so a crop CTA can never be running while a blend item it waits for has not even started);
-// a blend CTA, once its bulk store has completed, bumps the done-counter of every tile of its chain; a crop CTA polls
-// the counters of the tiles it depends on (job words CX0, CX1, CY0, FLAGS; -1 = none) against the number of blocks that
-// blend them (`expect`) before it issues its TMA loads.  Independent crops overlap the blends, the tail of one kernel and
-// the ramp of the next disappear, and a level costs two launches instead of three.  The last CTA to finish zeroes the
-// counters for the next launch.  Every wait gives up after ~1 s and raises the error word instead of hanging the GPU.
-struct LevelArgs {
-    const int32_t* tabs;
-    const uint8_t* mask_pool;
-    const int32_t* bjobs;      // blend job records (tensor-core flavour), word 31 = slot of the record's tile
-    const float* src;          // sampler output of wave k
-    const int32_t* cjobs;      // crop job records of wave k + 1
-    float* out;                // crop output
-    const int32_t* expect;     // per slot: canvas blocks that blend the tile
-    int* sync;                 // [0] ticket [1] finished CTAs [2] error [3 + slot * B + b] blocks done
-    int n_bheads, n_cjobs, B, W3;
-    int b_patch_w, b_plane_rows, b_mid_rows, block_rows;
-    int c_patch_w, c_plane_rows, c_mid_rows, n_slots;
-    CUtensorMap dmap;          // canvas as 192-byte x block_rows boxes (blend)
-    CUtensorMap cmap;          // canvas as 256-byte x 48-row boxes (crop)
-};
-
-__device__ __forceinline__ int ld_acquire(const int* p) {
-    int v;
-    asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-    return v;
-}
-__device__ __forceinline__ void fence_proxy_async_all() { asm volatile("fence.proxy.async;" ::: "memory"); }
-
-template <int KSMAX>
-__global__ void __launch_bounds__(kT, 3)
-level_mma_kernel(const __grid_constant__ LevelArgs a) {
-    extern __shared__ __align__(128) uint8_t smem[];
-    __shared__ int s_item;
-    pdl_launch_dependents();
-    pdl_wait();                                // everything this kernel touches comes from earlier kernels (counters included)
-    if (threadIdx.x == 0) s_item = atomicAdd(a.sync, 1);
-    __syncthreads();
-    const int item = s_item;
-    const int total = (a.n_bheads + a.n_cjobs) * a.B;
-    if (item < a.n_bheads * a.B) {
-        // ---------------- blend item: one canvas block of wave k (body of blend_mma_kernel<false>) ----------------
-        const int head = item / a.B, b = item - head * a.B;
-        const int block_rows = a.block_rows;
-        const size_t dbytes = (size_t)2 * block_rows * kDBox;
-        int32_t* job_sm = reinterpret_cast<int32_t*>(smem + dbytes);
-        uint64_t* bar = reinterpret_cast<uint64_t*>(smem + dbytes + kHeadBytes);
-        uint32_t* mid = reinterpret_cast<uint32_t*>(smem + dbytes + kHeadBytes + 16);
-        uint8_t* planes = smem + dbytes + kHeadBytes + 16 + mid_bytes(a.b_mid_rows);
-        const int PB = plane_pitch(a.b_patch_w);
-        const JobView J{job_sm};
-        DTile D{smem, block_rows};
-        int idx = head;
-        load_job(job_sm, a.bjobs, idx);
-        if (threadIdx.x == 0) tma::mbar_init(bar, 1);
-        __syncthreads();
-        const int bx3 = J[USDU_J_DST_X] * 3, by = J[USDU_J_DST_Y];
-        const bool two = bx3 + kDBox < a.W3;
-        if (threadIdx.x == 0) {
-            tma::mbar_expect_tx(bar, (uint32_t)(two ? dbytes : dbytes / 2));
-            tma::load_3d(smem, &a.dmap, bx3, by, b, bar);
-            if (two) tma::load_3d(smem + (size_t)block_rows * kDBox, &a.dmap, bx3 + kDBox, by, b, bar);
-        }
-        bool first = true;
-        while (idx >= 0) {
-            if (!first) {
-                __syncthreads();
-                load_job(job_sm, a.bjobs, idx);
-                __syncthreads();
-            }
-            const int64_t first_el = J.i64(USDU_J_SRC_A) + (int64_t)b * J.i64(USDU_J_FRAME_LO);
-            stage_f32(planes, PB, a.b_plane_rows, a.src + first_el, J[USDU_J_PITCH], J[USDU_J_ROWS], J[USDU_J_COLS]);
-            __syncthreads();
-            if (first) tma::mbar_wait(bar, 0);
-            if (J[USDU_J_FLAGS] & 1) {
-                BlendOpaque epi;
-                epi.d = D;
-                epi.nrows = J[USDU_J_ROWS_OUT];
-                both_passes<KSMAX>(planes, mid, a.tabs, J, PB, a.b_plane_rows, block_rows, epi);
-            } else {
-                BlendFeather epi;
-                epi.d = D;
-                epi.mpitch = J[USDU_J_MPITCH];
-                epi.mask = a.mask_pool + J.i64(USDU_J_OFF_LO);
-                epi.cx0 = J[USDU_J_CX0]; epi.cx1 = J[USDU_J_CX1];
-                epi.cy0 = J[USDU_J_CY0]; epi.cy1 = J[USDU_J_CY1];
-                both_passes<KSMAX>(planes, mid, a.tabs, J, PB, a.b_plane_rows, block_rows, epi);
-            }
-            idx = J[USDU_J_NEXT];
-            first = false;
-        }
-        tma::fence_async_smem();
-        __syncthreads();
-        if (threadIdx.x == 0) {
-            tma::store_3d(&a.dmap, bx3, by, b, smem);
-            if (two) tma::store_3d(&a.dmap, bx3 + kDBox, by, b, smem + (size_t)block_rows * kDBox);
-            tma::store_commit();
-            tma::store_wait_all();             // the block is IN the canvas, not merely read out of shared memory
-            fence_proxy_async_all();
-            __threadfence();
-            for (int i = head; i >= 0; i = __ldg(a.bjobs + (size_t)i * USDU_JOB_WORDS + USDU_J_NEXT))
-                atomicAdd(a.sync + 3 + __ldg(a.bjobs + (size_t)i * USDU_JOB_WORDS + USDU_J_SLOT) * a.B + b, 1);
-        }
-    } else {
-        // ---------------- crop item: one output block of a tile of wave k + 1 (body of crop_mma_kernel<1>) ----------------
-        const int j = item - a.n_bheads * a.B;
-        const int ci = j / a.B, b = j - ci * a.B;
-        const size_t region = max(mid_bytes(a.c_mid_rows), (size_t)2 * kBoxR * kBoxB);
-        uint32_t* mid = reinterpret_cast<uint32_t*>(smem);
-        uint8_t* raw = smem;
-        int32_t* job_sm = reinterpret_cast<int32_t*>(smem + region);
-        uint64_t* bar = reinterpret_cast<uint64_t*>(smem + region + kHeadBytes);
-        uint8_t* planes = smem + region + kHeadBytes + 16;
-        const int PB = plane_pitch(a.c_patch_w);
-        load_job(job_sm, a.cjobs, ci);
-        if (threadIdx.x == 0) tma::mbar_init(bar, 1);
-        __syncthreads();
-        const JobView J{job_sm};
-        const int sa3 = J[USDU_J_SRC_A] * 3;
-        if (threadIdx.x == 0) {
-            const int deps[4] = {J[USDU_J_CX0], J[USDU_J_CX1], J[USDU_J_CY0], J[USDU_J_FLAGS]};
-            for (int d = 0; d < 4; ++d) {
-                if (deps[d] < 0) continue;
-                const int need = __ldg(a.expect + deps[d]);
-                const int* ctr = a.sync + 3 + deps[d] * a.B + b;
-                unsigned spins = 0;
-                while (ld_acquire(ctr) < need) {
-                    __nanosleep(100);
-                    if (++spins > (1u << 23)) { atomicExch(a.sync + 2, 1); break; }   // ~1 s: report, do not hang
-                }
-            }
-            fence_proxy_async_all();           // the blocks were written through the async proxy of other SMs
-            const int x = sa3 & ~15, y = J[USDU_J_SRC_B];
-            const bool two = (sa3 - x) + J[USDU_J_COLS] * 3 > kBoxB && x + kBoxB < a.W3;
-            tma::mbar_expect_tx(bar, (two ? 2 : 1) * kBoxR * kBoxB);
-            tma::load_3d(raw, &a.cmap, x, y, b, bar);
-            if (two) tma::load_3d(raw + kBoxR * kBoxB, &a.cmap, x + kBoxB, y, b, bar);
-        }
-        tma::mbar_wait(bar, 0);
-        stage_raw(planes, PB, a.c_plane_rows, raw, J[USDU_J_ROWS], J[USDU_J_COLS], sa3 & 15);
-        __syncthreads();
-        CropEpilogue epi;
-        epi.row_pitch = J[USDU_J_PITCH];
-        epi.dst = a.out + J.i64(USDU_J_OFF_LO) + (int64_t)b * J.i64(USDU_J_FRAME_LO) + (int64_t)J[USDU_J_DST_Y] * epi.row_pitch +
-                  (int64_t)J[USDU_J_DST_X] * 3;
-        epi.ow3 = J[USDU_J_COLS_OUT] * 3;
-        epi.rows_out = J[USDU_J_ROWS_OUT];
-        both_passes<KSMAX>(planes, mid, a.tabs, J, PB, a.c_plane_rows, J[USDU_J_CY1], epi);
-    }
-    // the last CTA of the grid leaves ticket and counters at zero for the next launch (the error word stays)
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        __threadfence();
-        s_item = atomicAdd(a.sync + 1, 1);
-    }
-    __syncthreads();
-    if (s_item == total - 1) {
-        const int n = 3 + a.n_slots * a.B;
-        for (int i = threadIdx.x; i < n; i += kT)
-            if (i != 2) a.sync[i] = 0;
-        __threadfence();
-    }
-}
-
 static size_t crop_smem(int patch_w, int plane_rows, int mid_rows, bool use_tma) {
     const size_t region = use_tma ? max(mid_bytes(mid_rows), (size_t)2 * kBoxR * kBoxB) : mid_bytes(mid_rows);
     return region + kHeadBytes + 16 + planes_bytes(patch_w, plane_rows);
@@ -838,37 +668,6 @@ int launch_blend(uint8_t* canvas, int B, int H, int W, int64_t pitch, const int3
                           : launch_one(blend_mma_kernel<true, 1>, smem, grid, st, tabs, mask_pool, items, src, W3, patch_w, plane_rows, mid_rows, block_rows, cmap);
     return two_ksteps ? launch_one(blend_mma_kernel<false, 2>, smem, grid, st, tabs, mask_pool, items, src, W3, patch_w, plane_rows, mid_rows, block_rows, cmap)
                       : launch_one(blend_mma_kernel<false, 1>, smem, grid, st, tabs, mask_pool, items, src, W3, patch_w, plane_rows, mid_rows, block_rows, cmap);
-}
-
-int launch_level(uint8_t* canvas, int B, int H, int W, int64_t pitch, const int32_t* tabs, const uint8_t* mask_pool,
-                 const int32_t* bjobs, int n_bheads, int b_patch_w, int b_patch_h, const float* src, int block_rows,
-                 const int32_t* cjobs, int n_cjobs, int c_patch_w, int c_patch_h, float* out, const int32_t* expect, int n_slots,
-                 int* sync, int two_ksteps, cudaStream_t st) {
-    if (block_rows != 16 && block_rows != 32) {
-        set_error("usdu_level_blend_crop: block height must be 16 or 32, got %d", block_rows);
-        return USDU_ERR_INVALID;
-    }
-    LevelArgs a;
-    memset(&a, 0, sizeof(a));
-    int s = split_patch_h(b_patch_h, &a.b_plane_rows, &a.b_mid_rows, "usdu_level_blend_crop (blend)");
-    if (s != USDU_OK) return s;
-    s = split_patch_h(c_patch_h, &a.c_plane_rows, &a.c_mid_rows, "usdu_level_blend_crop (crop)");
-    if (s != USDU_OK) return s;
-    if (a.c_plane_rows > kBoxR || 12 + c_patch_w * 3 > 2 * kBoxB || ((uintptr_t)canvas & 15) != 0) {
-        set_error("usdu_level_blend_crop: the crop patch does not fit the TMA boxes (%d rows, %d px)", a.c_plane_rows, c_patch_w);
-        return USDU_ERR_UNSUPPORTED;
-    }
-    if (!tma::encode_u8_3d(&a.dmap, canvas, (uint64_t)W * 3, (uint64_t)H, (uint64_t)B, (uint64_t)pitch, kDBox, block_rows) ||
-        !tma::encode_u8_3d(&a.cmap, canvas, (uint64_t)W * 3, (uint64_t)H, (uint64_t)B, (uint64_t)pitch, kBoxB, kBoxR)) {
-        set_error("usdu_level_blend_crop: cannot build the canvas tensor maps (cuTensorMapEncodeTiled)");
-        return USDU_ERR_CUDA;
-    }
-    a.tabs = tabs; a.mask_pool = mask_pool; a.bjobs = bjobs; a.src = src; a.cjobs = cjobs; a.out = out; a.expect = expect; a.sync = sync;
-    a.n_bheads = n_bheads; a.n_cjobs = n_cjobs; a.B = B; a.W3 = W * 3;
-    a.b_patch_w = b_patch_w; a.block_rows = block_rows; a.c_patch_w = c_patch_w; a.n_slots = n_slots;
-    const size_t smem = max(blend_smem(b_patch_w, a.b_plane_rows, a.b_mid_rows, block_rows), crop_smem(c_patch_w, a.c_plane_rows, a.c_mid_rows, true));
-    const dim3 grid((unsigned)((n_bheads + n_cjobs) * B));
-    return two_ksteps ? launch_one(level_mma_kernel<2>, smem, grid, st, a) : launch_one(level_mma_kernel<1>, smem, grid, st, a);
 }
 
 }  // namespace mma

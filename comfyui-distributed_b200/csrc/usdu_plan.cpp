@@ -466,9 +466,8 @@ int kernel_path(const Plan* p, int path) {
 // Block edge of a launch.  `extents` = (width, height) in pixels each tile covers in the launch's block space.  The block
 // height is chosen by a simple wave model: cost(bh) = ceil(#CTAs / resident slots) * (bh + halo/fixed rows) -- short
 // blocks give small (latency bound) launches more CTAs, and large launches avoid a nearly empty last wave.
-// share = launches expected to run side by side: each gets 1/share of the machine.
 void block_shape(Plan* p, bool use_fast, const std::vector<std::pair<int64_t, int64_t>>& extents, int64_t frames,
-                 int64_t share, bool mma, const LaunchModel& m, int& bw_out, int& bh_out) {
+                 bool mma, const LaunchModel& m, int& bw_out, int& bh_out) {
     if (!use_fast) {
         p->generic_block(bw_out, bh_out);
         return;
@@ -492,7 +491,7 @@ void block_shape(Plan* p, bool use_fast, const std::vector<std::pair<int64_t, in
         int64_t n = 0;
         for (const auto& e : extents) n += (floordiv(e.first + bw - 1, bw) + 1) * (floordiv(e.second + bh - 1, bh) + 1);   // +1: unaligned windows
         n *= frames;
-        const int64_t cost = (int64_t)ceil((double)n / (double)std::max(floordiv(slots, std::max(share, (int64_t)1)), (int64_t)1)) * (bh + 12);
+        const int64_t cost = (int64_t)ceil((double)n / (double)std::max(slots, (int64_t)1)) * (bh + 12);
         if (!have || cost < best_cost || (cost == best_cost && bh > best_bh)) {
             have = true;
             best_cost = cost;
@@ -569,7 +568,7 @@ int check_ids(const Plan* p, const int32_t* ids, int n, const char* what) {
     return USDU_OK;
 }
 
-int crop_worklist(Plan* p, const int32_t* ids, int n, int B, int req_path, int share, const LaunchModel& m, WorkList* wl) {
+int crop_worklist(Plan* p, const int32_t* ids, int n, int B, int req_path, const LaunchModel& m, WorkList* wl) {
     const int path = kernel_path(p, req_path);
     const bool use_fast = path >= 1;
     wl->slots.resize(n);
@@ -583,7 +582,7 @@ int crop_worklist(Plan* p, const int32_t* ids, int n, int B, int req_path, int s
     std::vector<std::pair<int64_t, int64_t>> ext;
     for (int i = 0; i < n; ++i) ext.emplace_back(p->tiles[ids[i]].pw - USDU_FAST_BLOCK_W, p->tiles[ids[i]].ph);
     int bw, bh_max;
-    block_shape(p, use_fast, ext, B, share, path == 2, m, bw, bh_max);
+    block_shape(p, use_fast, ext, B, path == 2, m, bw, bh_max);
     std::vector<int64_t> items;     // generic items [tile, ox0, oy0, off_lo, off_hi, bh]
     int64_t pw_max = 1, ph_max = 1, nbytes = 0;
     for (int i = 0; i < n; ++i) {
@@ -689,21 +688,12 @@ int crop_worklist(Plan* p, const int32_t* ids, int n, int B, int req_path, int s
     return USDU_OK;
 }
 
-// numpy's slice bounds [start:stop] on an axis of n elements
-void py_slice(int64_t n, int64_t& start, int64_t& stop) {
-    if (start < 0) start += n;
-    if (stop < 0) stop += n;
-    start = clip(start, 0, n);
-    stop = clip(stop, 0, n);
-}
-
 struct Pair {
     int64_t key, seq, tid;
 };
 
 int blend_worklist(Plan* p, const int32_t* ids, const int64_t* offs, int n, int src_bytes, int B, int req_path,
-                   int part_i, int part_n, int share, const int64_t* rects, int n_rects, int keep, const LaunchModel& m,
-                   WorkList* wl) {
+                   int part_i, int part_n, const LaunchModel& m, WorkList* wl) {
     const int path = kernel_path(p, req_path);
     const bool use_fast = path >= 1;
     std::vector<std::pair<int64_t, int64_t>> ext;
@@ -713,7 +703,7 @@ int blend_worklist(Plan* p, const int32_t* ids, const int64_t* offs, int n, int 
         ext.emplace_back(s[2] - s[0], s[3] - s[1]);
     }
     int bw_, bh_;
-    block_shape(p, use_fast, ext, B, share, path == 2, m, bw_, bh_);
+    block_shape(p, use_fast, ext, B, path == 2, m, bw_, bh_);
     const int64_t bw = bw_, bh = bh_, W = p->W, H = p->H;
     const int64_t nbx = (W + bw - 1) / bw, nby = (H + bh - 1) / bh;
     int64_t lo_b = 0, hi_b = 0;
@@ -722,22 +712,6 @@ int blend_worklist(Plan* p, const int32_t* ids, const int64_t* offs, int n, int 
         hi_b = (nby * (part_i + 1)) / part_n;
         wl->row0 = std::min(lo_b * bh, H);
         wl->row1 = std::min(hi_b * bh, H);
-    }
-    std::vector<uint8_t> sel;
-    if (keep >= 0) {
-        std::vector<uint8_t> hit((size_t)(nby * nbx), 0);
-        for (int r = 0; r < n_rects; ++r) {
-            const int64_t rx0 = rects[4 * r], ry0 = rects[4 * r + 1], rx1 = rects[4 * r + 2], ry1 = rects[4 * r + 3];
-            if (!(rx1 > rx0 && ry1 > ry0)) continue;
-            int64_t y0 = floordiv(std::max(ry0, (int64_t)0), bh), y1 = floordiv(std::min(ry1, H) - 1, bh) + 1;
-            int64_t x0 = floordiv(std::max(rx0, (int64_t)0), bw), x1 = floordiv(std::min(rx1, W) - 1, bw) + 1;
-            py_slice(nby, y0, y1);
-            py_slice(nbx, x0, x1);
-            for (int64_t gy = y0; gy < y1; ++gy)
-                for (int64_t gx = x0; gx < x1; ++gx) hit[gy * nbx + gx] = 1;
-        }
-        sel.resize(hit.size());
-        for (size_t k = 0; k < hit.size(); ++k) sel[k] = keep ? hit[k] : !hit[k];
     }
     std::vector<Pair> pairs;
     int64_t pw_max = 1, ph_max = 1, nbytes = 0;
@@ -754,20 +728,11 @@ int blend_worklist(Plan* p, const int32_t* ids, const int64_t* offs, int n, int 
             gy1 = std::min(gy1, hi_b);
             if (gy1 <= gy0) continue;
         }
-        const int64_t n_all = (gy1 - gy0) * std::max(gx1 - gx0, (int64_t)0);
-        int64_t kept = 0;
         for (int64_t gy = gy0; gy < gy1; ++gy)
-            for (int64_t gx = gx0; gx < gx1; ++gx) {
-                const int64_t k = gy * nbx + gx;
-                if (!sel.empty() && !sel[k]) continue;
-                pairs.push_back({k, s, ids[s]});
-                ++kept;
-            }
-        if (!sel.empty() && kept == 0) continue;
+            for (int64_t gx = gx0; gx < gx1; ++gx) pairs.push_back({gy * nbx + gx, s, ids[s]});
         pw_max = std::max(pw_max, p->span_max(p->tables[t.tab_blend_h], bw, false));
         ph_max = std::max(ph_max, p->span_max(p->tables[t.tab_blend_v], bh, false));
-        const double frac = (part_n <= 0 ? 1.0 : (double)((gy1 - gy0) * bh) / (double)std::max(Y1 - Y0, (int64_t)1)) *
-                            ((double)kept / (double)std::max(n_all, (int64_t)1));
+        const double frac = part_n <= 0 ? 1.0 : (double)((gy1 - gy0) * bh) / (double)std::max(Y1 - Y0, (int64_t)1);
         nbytes += (int64_t)(std::min(frac, 1.0) * (double)(t.pw * t.ph * 3 * src_bytes + 2 * (sp[2] - sp[0]) * (sp[3] - sp[1]) * 3));
     }
     wl->path = path;
@@ -860,7 +825,6 @@ int blend_worklist(Plan* p, const int32_t* ids, const int64_t* offs, int n, int 
         r[USDU_J_FLAGS] = opaque ? 1 : 0;
         r[USDU_J_MPITCH] = mpitch;
         set_frame(r, t.pw, t.ph);
-        r[USDU_J_SLOT] = q.seq;                 // position of the record's tile in the launch's tile list
     }
     // record order: heads (one per block) first, then the rest; chain through NEXT
     std::vector<int64_t> pos(np);
@@ -1087,7 +1051,7 @@ int usdu_plan_waves(const usdu_plan* plan, const int32_t* order, int n, int32_t*
     });
 }
 
-int usdu_plan_crop_worklist(const usdu_plan* plan, const int32_t* tile_ids, int n, int B, int path, int share, int sm_count,
+int usdu_plan_crop_worklist(const usdu_plan* plan, const int32_t* tile_ids, int n, int B, int path, int sm_count,
                             int mma_block_rows, usdu_worklist** wl) {
     const Plan* p = reinterpret_cast<const Plan*>(plan);
     USDU_PLAN_ARG(p);
@@ -1105,7 +1069,7 @@ int usdu_plan_crop_worklist(const usdu_plan* plan, const int32_t* tile_ids, int 
     return guarded([&]() {
         WorkList* w = new WorkList();
         // the plan caches its generic block shape: a pure function of the plan
-        const int r = crop_worklist(const_cast<Plan*>(p), tile_ids, n, B, path, share, LaunchModel{sm_count, mma_block_rows}, w);
+        const int r = crop_worklist(const_cast<Plan*>(p), tile_ids, n, B, path, LaunchModel{sm_count, mma_block_rows}, w);
         if (r != USDU_OK) {
             delete w;
             return r;
@@ -1116,8 +1080,7 @@ int usdu_plan_crop_worklist(const usdu_plan* plan, const int32_t* tile_ids, int 
 }
 
 int usdu_plan_blend_worklist(const usdu_plan* plan, const int32_t* tile_ids, const int64_t* src_offsets, int n, int src_bytes,
-                             int B, int path, int part_i, int part_n, int share, const int64_t* select_rects, int n_rects,
-                             int select_keep, int sm_count, int mma_block_rows, usdu_worklist** wl) {
+                             int B, int path, int part_i, int part_n, int sm_count, int mma_block_rows, usdu_worklist** wl) {
     const Plan* p = reinterpret_cast<const Plan*>(plan);
     USDU_PLAN_ARG(p);
     if (!wl) {
@@ -1128,17 +1091,16 @@ int usdu_plan_blend_worklist(const usdu_plan* plan, const int32_t* tile_ids, con
     int s = check_ids(p, tile_ids, n, "usdu_plan_blend_worklist");
     if (s != USDU_OK) return s;
     if ((n > 0 && !src_offsets) || (src_bytes != 1 && src_bytes != 4) || B <= 0 || path < 0 || part_n < 0 ||
-        (part_n > 0 && (part_i < 0 || part_i >= part_n)) || n_rects < 0 || (n_rects > 0 && !select_rects) || sm_count < 0 ||
-        mma_block_rows < 0 || mma_block_rows > USDU_FAST_BLOCK_H || select_keep < -1 || select_keep > 1) {
-        usdu::set_error("usdu_plan_blend_worklist: bad arguments (src_bytes=%d B=%d path=%d part=%d/%d n_rects=%d keep=%d "
-                        "sm_count=%d mma_block_rows=%d)", src_bytes, B, path, part_i, part_n, n_rects, select_keep, sm_count,
-                        mma_block_rows);
+        (part_n > 0 && (part_i < 0 || part_i >= part_n)) || sm_count < 0 || mma_block_rows < 0 ||
+        mma_block_rows > USDU_FAST_BLOCK_H) {
+        usdu::set_error("usdu_plan_blend_worklist: bad arguments (src_bytes=%d B=%d path=%d part=%d/%d sm_count=%d "
+                        "mma_block_rows=%d)", src_bytes, B, path, part_i, part_n, sm_count, mma_block_rows);
         return USDU_ERR_INVALID;
     }
     return guarded([&]() {
         WorkList* w = new WorkList();
-        const int r = blend_worklist(const_cast<Plan*>(p), tile_ids, src_offsets, n, src_bytes, B, path, part_i, part_n, share,
-                                     select_rects, n_rects, select_keep, LaunchModel{sm_count, mma_block_rows}, w);
+        const int r = blend_worklist(const_cast<Plan*>(p), tile_ids, src_offsets, n, src_bytes, B, path, part_i, part_n,
+                                     LaunchModel{sm_count, mma_block_rows}, w);
         if (r != USDU_OK) {
             delete w;
             return r;

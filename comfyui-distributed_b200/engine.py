@@ -76,11 +76,6 @@ PATH_FLAGS = (0, nat.FLAG_FAST, nat.FLAG_MMA)
 _PATHS = {"generic": 0, "fast": 1, "mma": 2}
 PATH_CROP = _PATHS[os.environ.get("USDU_CROP_PATH", "mma")]      # best build per kernel (upper bound: the plan may not support it)
 PATH_BLEND = _PATHS[os.environ.get("USDU_BLEND_PATH", "mma")]
-# blend(k) and crop(k+1) in ONE launch with device-side ready counters (usdu_level_blend_crop).  Correct (full-size digests,
-# 114 GPU tests) but not faster than the level loop with a T0-cost sampler:
-# a crop of wave k+1 needs whole TILES of wave k, whose blocks finish late in the grid, so little overlaps, while every blend
-# CTA now waits for its bulk store to COMPLETE and the grid runs at the larger of the two shared-memory footprints.  Off by default.
-FUSE_LEVELS = os.environ.get("USDU_FUSE_LEVELS", "0") == "1"
 USE_CUDA_GRAPHS = True    # capture the wave loop when the sampler is cuda_graph_safe
 
 
@@ -118,64 +113,43 @@ class DevicePlan:
         cover = torch.from_numpy(wl.cover).to(self.device) if wl.cover is not None else None
         return items, cover
 
-    def crop_list(self, tile_ids: Tuple[int, ...], B: int, use_fast: bool, share: int = 1):
-        key = ("crop", tile_ids, B, use_fast, share)
+    def crop_list(self, tile_ids: Tuple[int, ...], B: int, use_fast: bool):
+        key = ("crop", tile_ids, B, use_fast)
         if key not in self._wl:
-            wl, offs, total = self.plan.crop_worklist(tile_ids, B, use_fast, share)
+            wl, offs, total = self.plan.crop_worklist(tile_ids, B, use_fast)
             self._wl[key] = (wl, offs, total) + self._upload(wl)
         return self._wl[key]
 
     def blend_list(self, tile_ids: Tuple[int, ...], offs: np.ndarray, src_u8: bool, use_fast: bool, B: int = 1,
-                   part: Optional[Tuple[int, int]] = None, share: int = 1):
-        key = ("blend", tile_ids, tuple(int(o) for o in offs), src_u8, use_fast, B, part, share)
+                   part: Optional[Tuple[int, int]] = None):
+        key = ("blend", tile_ids, tuple(int(o) for o in offs), src_u8, use_fast, B, part)
         if key not in self._wl:
-            wl = self.plan.blend_worklist(tile_ids, offs, 1 if src_u8 else 4, use_fast, B, part, share)
+            wl = self.plan.blend_worklist(tile_ids, offs, 1 if src_u8 else 4, use_fast, B, part)
             self._wl[key] = (wl,) + self._upload(wl)
         return self._wl[key]
 
     def split_lists(self, waves: Sequence[Sequence[int]], B: int, path_crop: int, path_blend: int):
         """Per dependency wave, the work lists of the split schedule (planner.split_level), uploaded:
-        dict(crop=(wl, items), early / late = (wl, items) or None, offs, total, crit=(wl, items), rest=(wl, items) or None),
+        dict(crop=(wl, items), early / late = (wl, items) or None, offs, total, blend=(wl, items)),
         or None when some wave does not run on job records."""
         key = ("split", tuple(tuple(int(t) for t in w) for w in waves), B, path_crop, path_blend)
         if key not in self._wl:
             out = []
             for k, wave in enumerate(waves):
                 offs, _ = self.plan.slot_offsets(wave, B)
-                nxt = waves[k + 1] if k + 1 < len(waves) else None
-                prev = waves[k - 1] if k else None
-                # (the crop lists decide which blend blocks are critical: both sides use the crop path of the launch)
-                cr, coffs, ctotal, late, crit, rest = self.plan.split_level(wave, offs, nxt, prev, B, path_crop)
+                cr, coffs, ctotal, late, bl = self.plan.split_level(wave, offs, waves[k - 1] if k else None, B, path_crop)
                 if path_blend != path_crop:
-                    crit = self.plan.blend_worklist(wave, offs, 4, path_blend, B)
-                    rest = None
-                if cr.path < 1 or crit.path < 1:
+                    bl = self.plan.blend_worklist(wave, offs, 4, path_blend, B)
+                if cr.path < 1 or bl.path < 1:
                     out = None
                     break
                 e = {"crop": (cr, self._upload(cr)[0]), "offs": coffs, "total": ctotal, "early": None, "late": None,
-                     "crit": (crit, self._upload(crit)[0]), "rest": None}
-                full = crit if rest is None else self.plan.blend_worklist(wave, offs, 4, path_blend, B)
-                e["full"] = e["crit"] if rest is None else (full, self._upload(full)[0])
+                     "blend": (bl, self._upload(bl)[0])}
                 if late is not None and late.any() and not late.all():
                     we, wlate = self.plan.sub_worklist(cr, ~late), self.plan.sub_worklist(cr, late)
                     e["early"], e["late"] = (we, self._upload(we)[0]), (wlate, self._upload(wlate)[0])
-                if rest is not None and rest.n_launch > 0 and crit.n_launch > 0:
-                    e["rest"] = (rest, self._upload(rest)[0])
-                elif rest is not None and crit.n_launch <= 0:
-                    e["crit"] = (rest, self._upload(rest)[0])
                 out.append(e)
             self._wl[key] = out
-        return self._wl[key]
-
-    def level_list(self, blend_ids: Tuple[int, ...], offs: np.ndarray, crop_ids: Tuple[int, ...], B: int, share: int = 1):
-        key = ("level", blend_ids, tuple(int(o) for o in offs), crop_ids, B, share)
-        if key not in self._wl:
-            r = self.plan.level_worklist(blend_ids, offs, crop_ids, B, share)
-            if r is not None:
-                bl, cr, coffs, ctotal, expect = r
-                r = (bl, cr, coffs, ctotal, torch.from_numpy(bl.items).to(self.device), torch.from_numpy(cr.items).to(self.device),
-                     torch.from_numpy(expect).to(self.device))
-            self._wl[key] = r
         return self._wl[key]
 
 
@@ -202,8 +176,6 @@ class Canvas:
         # both give identical bytes
         self.path_crop = min(self.path, PATH_CROP)
         self.path_blend = min(self.path, PATH_BLEND)
-        self.share = 1                      # launches expected to run side by side (tile-granular schedule)
-        self._sync = None                   # ticket + per-tile counters of the fused level launches (left at zero by the kernel)
 
     @staticmethod
     def pitch_of(W: int) -> int:
@@ -250,7 +222,7 @@ class Canvas:
         image: crop the windows straight from this fp32 image [B,H,W,3] instead of the canvas (identical tiles as long
         as the canvas still is the quantised image there: a conflict-free partition, dist.StaticJob)."""
         tile_ids = tuple(int(t) for t in tile_ids)
-        wl, offs, total, items, _ = self.dp.crop_list(tile_ids, self.B, self.path_crop, self.share)
+        wl, offs, total, items, _ = self.dp.crop_list(tile_ids, self.B, self.path_crop)
         if image is not None:
             if not (self.can_crop_image() and wl.path == 2):
                 raise nat.NativeError("crop from the fp32 image needs the tensor-core kernels and a canvas width that is a multiple of 4")
@@ -298,8 +270,7 @@ class Canvas:
         if src.dtype not in (torch.float32, torch.uint8):
             raise ValueError(f"blend: src must be float32 or uint8, got {src.dtype}")
         src_u8 = src.dtype == torch.uint8
-        wl, items, cover = self.dp.blend_list(tile_ids, offs, src_u8, self.path_blend, self.B, part,
-                                              1 if part is not None else self.share)
+        wl, items, cover = self.dp.blend_list(tile_ids, offs, src_u8, self.path_blend, self.B, part)
         self.blend_jobs(wl, items, cover, src, canvas_ptr)
 
     def blend_jobs(self, wl: WorkList, items: torch.Tensor, cover: Optional[torch.Tensor], src: torch.Tensor,
@@ -323,37 +294,6 @@ class Canvas:
                                        src_u8, flags, _stream_ptr()))
         self.launches += 1
         self.algo_bytes += wl.algo_bytes * self.B
-
-
-def _canvas_blend_crop(self, blend_ids: Sequence[int], src: torch.Tensor, offs: np.ndarray, crop_ids: Sequence[int]):
-    """ONE launch: composite the processed tiles `blend_ids` (fp32 sampler output `src`) AND crop the tiles `crop_ids` of
-    the next dependency wave, ordered on the device tile by tile (usdu_level_blend_crop).  -> (crop buffer, crop offsets)
-    or None when the launch does not qualify (the caller then issues the two launches)."""
-    if not (FUSE_LEVELS and self.path_crop == 2 and self.path_blend == 2 and src.dtype == torch.float32):
-        return None
-    blend_ids, crop_ids = tuple(int(t) for t in blend_ids), tuple(int(t) for t in crop_ids)
-    r = self.dp.level_list(blend_ids, offs, crop_ids, self.B, self.share)
-    if r is None:
-        return None
-    bl, cr, coffs, ctotal, bitems, citems, expect = r
-    need = 3 + len(blend_ids) * self.B
-    if self._sync is None or self._sync.numel() < need:
-        self._sync = torch.zeros(max(need, 64), dtype=torch.int32, device=self.buf.device)
-    out = torch.empty(ctotal, dtype=torch.float32, device=self.buf.device)
-    p = self.plan
-    src = src.contiguous()
-    flags = nat.FLAG_MMA | (nat.FLAG_MMA_KS2 if (bl.ks2 or cr.ks2) else 0)
-    _launch("level(blend+crop)", (bl.algo_bytes + cr.algo_bytes) * self.B,
-            lambda: nat.level_blend_crop(self.buf.data_ptr(), self.B, p.H, p.W, self.pitch, self.dp.tabs.data_ptr(),
-                                         self.dp.mask_pool.data_ptr(), bitems.data_ptr(), bl.n_launch, bl.patch_w, bl.patch_h,
-                                         src.data_ptr(), bl.block_rows, citems.data_ptr(), citems.shape[0], cr.patch_w, cr.patch_h,
-                                         out.data_ptr(), expect.data_ptr(), len(blend_ids), self._sync.data_ptr(), flags, _stream_ptr()))
-    self.launches += 1
-    self.algo_bytes += (bl.algo_bytes + cr.algo_bytes) * self.B
-    return out, coffs
-
-
-Canvas.blend_crop = _canvas_blend_crop
 
 
 def tile_views(plan: Plan, tile_ids: Sequence[int], buf: torch.Tensor, offs: np.ndarray, B: int):
@@ -417,12 +357,8 @@ def run_progressive(canvas: Canvas, order: Sequence[int], denoiser: Denoiser, ke
     shipped: Dict[int, torch.Tensor] = {}
     scratch = None
     waves = [_sorted_by_shape(plan, w) for w in plan.waves(order)]
-    fused = None                                   # (crop buffer, offsets) of this wave when the previous level launch made it
-    for k, wave in enumerate(waves):
-        if fused is not None:
-            buf, offs = fused
-            fused = None
-        elif "crop" in skip and crop_buf is not None:    # the caller cropped this (single) wave itself: GraphedWaves.replay_from_image
+    for wave in waves:
+        if "crop" in skip and crop_buf is not None:    # the caller cropped this (single) wave itself: GraphedWaves.replay_from_image
             offs, total = plan.slot_offsets(wave, B)
             buf = crop_buf[:total]
         elif "crop" in skip:    # bench.py's differencing measurement: same graph minus one kernel kind
@@ -434,10 +370,7 @@ def run_progressive(canvas: Canvas, order: Sequence[int], denoiser: Denoiser, ke
             buf, offs = canvas.crop(wave)
         out = denoise_packed(plan, wave, buf, offs, B, denoiser)
         if "blend" not in skip:
-            if not skip and k + 1 < len(waves):    # blend(k) U crop(k+1) as one launch, ordered on the device
-                fused = canvas.blend_crop(wave, out, offs, waves[k + 1])
-            if fused is None:
-                canvas.blend(wave, out, offs)
+            canvas.blend(wave, out, offs)
         if payload is not None:
             sizes = [B * plan.tiles[t].ph * plan.tiles[t].pw * 3 for t in wave]
             base = where[wave[0]][1]
@@ -462,65 +395,12 @@ def run_progressive(canvas: Canvas, order: Sequence[int], denoiser: Denoiser, ke
     return shipped
 
 
-# waves | split_crop (default: waves whose crop launches are split by what they really depend on, run_split) | split_blend | split |
-# split_crop_a | split_crop_b | dag
+# split_crop (default: waves whose crop launches are split by what they really depend on, run_split) | waves (the plain
+# level loop, run_progressive)
 SCHEDULE = os.environ.get("USDU_SCHEDULE", "split_crop")
-SCHEDULES = ("waves", "split_crop", "split_crop_a", "split_crop_b", "split_blend", "split", "dag")
+SCHEDULES = ("waves", "split_crop")
 if SCHEDULE not in SCHEDULES:
     raise ValueError(f"USDU_SCHEDULE={SCHEDULE!r}: expected one of {', '.join(SCHEDULES)}")
-
-
-def use_dag(plan: Plan, order: Sequence[int]) -> bool:
-    """Level waves (with split crops, run_split) by default.  The tile-granular schedule (USDU_SCHEDULE=dag) shortens the critical path from 31
-    waves to 31 single-tile chains, but with a T0-cost sampler its 405 graph kernel nodes on 9 streams are bound by
-    the launch rate of the graph, not by the chain.  It pays only when the sampler call is long enough to hide node launches but too small to
-    fill the machine with one tile."""
-    return SCHEDULE == "dag" and len(plan.waves(order)) > 2
-
-
-def run_dag(canvas: Canvas, order: Sequence[int], denoiser: Denoiser, lanes: List["torch.cuda.Stream"],
-            payload: Optional[torch.Tensor] = None, where: Optional[dict] = None, skip: Sequence[str] = ()):
-    """The same job as run_progressive(order) as a tile-granular DAG (planner.Plan.dag): one crop -> sampler ->
-    blend chain per tile, chains on `lanes` (CUDA streams) joined by events only where covers intersect.  Meant to
-    be stream-captured (GraphedWaves): level k+1's crops then overlap level k's blends of unrelated tiles, and the
-    critical path is 31 single-tile chains instead of 31 whole waves (single_gpu.py:40-64 fixes only the ORDER of
-    overlapping tiles).  The caller's current stream forks into the lanes and joins them at the end."""
-    plan, B = canvas.plan, canvas.B
-    order = [int(t) for t in order]
-    lane_of, waits = plan.dag(order)
-    main = torch.cuda.current_stream(canvas.buf.device)
-    fork = torch.cuda.Event()
-    fork.record(main)
-    used = sorted(set(lane_of))
-    for ln in used:
-        lanes[ln].wait_event(fork)
-    waited = {w for ws in waits for w in ws}
-    done: Dict[int, torch.cuda.Event] = {}
-    canvas.share = max(1, min(len(used), 16))
-    try:
-        for i, tid in enumerate(order):
-            st = lanes[lane_of[i]]
-            for w in waits[i]:
-                st.wait_event(done[w])
-            with torch.cuda.stream(st):
-                if "crop" in skip:
-                    offs, total = plan.slot_offsets([tid], B)
-                    buf = torch.empty(total, dtype=torch.float32, device=canvas.buf.device)   # timing variant: contents unused
-                else:
-                    buf, offs = canvas.crop([tid])
-                out = denoise_packed(plan, [tid], buf, offs, B, denoiser)
-                if "blend" not in skip:
-                    canvas.blend([tid], out, offs)
-                if payload is not None:
-                    nat.pack_tiles_u8(out.data_ptr(), payload[where[tid][1]:].data_ptr(), out.numel(), _stream_ptr())
-                    canvas.launches += 1
-                if i in waited:
-                    done[i] = torch.cuda.Event()
-                    done[i].record(st)
-    finally:
-        canvas.share = 1
-    for ln in used:
-        main.wait_stream(lanes[ln])
 
 
 # The canvas quantise / dequantise of a graphed 1-GPU job as row bands inside the wave graph (CastBands, run_split), beside
@@ -604,26 +484,20 @@ class CastBands:
 
 
 def use_split(canvas: Canvas, order: Sequence[int]) -> bool:
-    """USDU_SCHEDULE=split*: level waves whose crop (and blend) launches are split by what the NEXT level really needs."""
-    return SCHEDULE.startswith("split") and not FUSE_LEVELS and canvas.path_crop >= 1 and canvas.path_blend >= 1 and len(canvas.plan.waves(order)) > 2
+    """USDU_SCHEDULE=split_crop: level waves whose crop launches are split by what they really depend on."""
+    return SCHEDULE == "split_crop" and canvas.path_crop >= 1 and canvas.path_blend >= 1 and len(canvas.plan.waves(order)) > 2
 
 
-def run_split(canvas: Canvas, order: Sequence[int], denoiser: Denoiser, s_rest: "torch.cuda.Stream",
-              s_early: "torch.cuda.Stream", skip: Sequence[str] = (), casts: Optional[CastBands] = None) -> bool:
-    """run_progressive(order) with every level's two launches split by dependency (planner.split_level); meant to be
+def run_split(canvas: Canvas, order: Sequence[int], denoiser: Denoiser, s_early: "torch.cuda.Stream",
+              casts: Optional[CastBands] = None) -> bool:
+    """run_progressive(order) with every level's crop launch split by dependency (planner.split_level); meant to be
     stream-captured.  single_gpu.py:40-64 orders a crop only after the blends that CHANGE pixels it reads:
-      * crop(k+1) = `late` jobs (their staged rectangle meets a feather support of wave k) + `early` jobs, which run on
-        `s_early` beside sampler(k) / blend(k);
-      * blend(k)  = `crit` blocks (read by a late crop job of wave k+1) + `rest`, which runs on `s_rest` beside crop_late(k+1)
-        and sampler(k+1) and only has to land before blend(k+1) and crop_early(k+2).
-    The chain per level shrinks to crop_late -> sampler -> blend_crit (about a quarter of the crop jobs and a third of the
-    blend blocks on cfg2).  Blocks are owned by one blend launch at a time (a blend rewrites whole blocks), two launches
-    that run side by side never write the same block, and a crop beside a blend only ever reads bytes whose value the
-    blend leaves as it is.  False (nothing launched) when a wave has no job-record lists.
-    SCHEDULE: "split_crop" (default) splits only the crops; "split_blend" and "split" (both) also split the blends,
-    whose join takes the programmatic edge away from the critical blend.  skip: bench.py's differencing measurement -- the same schedule minus one kernel kind.
-    casts: the canvas quantise / dequantise bands (CastBands, split_crop only) run inside the same graph: a crop waits
-    for the quantise bands it reads, a dequantise band forks after the last blend that writes its rows."""
+    crop(k+1) = `late` jobs (their staged rectangle meets a feather support of wave k) + `early` jobs, which run on
+    `s_early` beside sampler(k) / blend(k).  The chain per level shrinks to crop_late -> sampler -> blend (about a quarter
+    of the crop jobs on cfg2).  A crop beside a blend only ever reads bytes whose value the blend leaves as it is.
+    False (nothing launched) when a wave has no job-record lists.
+    casts: the canvas quantise / dequantise bands (CastBands) run inside the same graph: a crop waits for the quantise
+    bands it reads, a dequantise band forks after the last blend that writes its rows."""
     plan, B = canvas.plan, canvas.B
     waves = [_sorted_by_shape(plan, w) for w in plan.waves(order)]
     lists = canvas.dp.split_lists(waves, B, canvas.path_crop, canvas.path_blend)
@@ -631,84 +505,39 @@ def run_split(canvas: Canvas, order: Sequence[int], denoiser: Denoiser, s_rest: 
         return False
     dev = canvas.buf.device
     main = torch.cuda.current_stream(dev)
-
-    def event(stream):
-        e = torch.cuda.Event()
-        e.record(stream)
-        return e
-
-    split_crop, split_blend = SCHEDULE != "split_blend", not SCHEDULE.startswith("split_crop")
-    # where the early crops of wave k+1 fork off: 0 = right after blend(k-1), 1 = after crop_late(k), 2 = after sampler(k)
-    # (with a split blend they must wait for blend_rest(k-1): 2)
-    fork_at = {"split_crop_a": 0, "split_crop_b": 1}.get(SCHEDULE, 2)
-    no_crop, no_blend = "crop" in skip, "blend" in skip
-    if not split_crop or no_crop:
-        lists = [dict(e, early=None, late=None) for e in lists]
-    if not split_blend:
-        lists = [dict(e, crit=e["full"], rest=None) for e in lists]
     bufs = [None] * len(waves)
     early_done = [None] * len(waves)
-    rest_done = None
-    keep = []                                     # tensors another stream still reads: released at the joins
-    new_buf = torch.zeros if no_crop else torch.empty
-    bufs[0] = new_buf(lists[0]["total"], dtype=torch.float32, device=dev)
+    bufs[0] = torch.empty(lists[0]["total"], dtype=torch.float32, device=dev)
     if casts is not None:
-        if SCHEDULE != "split_crop" or skip:
-            raise ValueError("canvas cast bands run only with the split_crop schedule")
         casts.start(canvas, main)
-
-    def fork_early(k):                            # the crop jobs of wave k+1 that do not read what wave k changes
-        if k + 1 < len(waves):
+    for k, wave in enumerate(waves):
+        L = lists[k]
+        buf = bufs[k]
+        if casts is not None:
+            casts.need(k, main)
+        if early_done[k] is not None:
+            canvas.crop_jobs(L["late"][0], L["late"][1], buf)
+            main.wait_event(early_done[k])
+        else:
+            canvas.crop_jobs(L["crop"][0], L["crop"][1], buf)
+        out = denoise_packed(plan, wave, buf, L["offs"], B, denoiser)
+        if k + 1 < len(waves):                    # the crop jobs of wave k+1 that do not read what wave k changes
             N = lists[k + 1]
-            bufs[k + 1] = new_buf(N["total"], dtype=torch.float32, device=dev)
+            bufs[k + 1] = torch.empty(N["total"], dtype=torch.float32, device=dev)
             if N["early"] is not None:
-                s_early.wait_event(event(main))
+                fork = torch.cuda.Event()
+                fork.record(main)
+                s_early.wait_event(fork)
                 if casts is not None:
                     casts.need(k + 1, s_early)
                 with torch.cuda.stream(s_early):
                     canvas.crop_jobs(N["early"][0], N["early"][1], bufs[k + 1])
-                    early_done[k + 1] = event(s_early)
-
-    for k, wave in enumerate(waves):
-        L = lists[k]
-        if fork_at == 0:
-            fork_early(k)
-        buf, offs = bufs[k], L["offs"]
-        if casts is not None:
-            casts.need(k, main)
-        if L["late"] is not None and early_done[k] is not None:
-            canvas.crop_jobs(L["late"][0], L["late"][1], buf)
-            if fork_at == 1:
-                fork_early(k)
-            main.wait_event(early_done[k])
-        else:
-            if not no_crop:
-                canvas.crop_jobs(L["crop"][0], L["crop"][1], buf)
-            if fork_at == 1:
-                fork_early(k)
-        out = denoise_packed(plan, wave, buf, offs, B, denoiser)
-        if L["rest"] is not None and not no_blend:    # the blocks no crop of the next wave waits for: beside the next level
-            s_rest.wait_event(event(main))
-            with torch.cuda.stream(s_rest):
-                canvas.blend_jobs(L["rest"][0], L["rest"][1], None, out)
-                this_rest = event(s_rest)
-        else:
-            this_rest = None
-        if rest_done is not None:                 # blend_rest(k-1) has landed: blocks change hands, early crops may read them
-            main.wait_event(rest_done)
-            keep.clear()
-        if this_rest is not None:
-            keep.append(out)                      # blend_rest(k) reads it on the other stream until the next join
-        rest_done = this_rest
-        if fork_at == 2:
-            fork_early(k)
-        if not no_blend:
-            canvas.blend_jobs(L["crit"][0], L["crit"][1], None, out)
+                    early_done[k + 1] = torch.cuda.Event()
+                    early_done[k + 1].record(s_early)
+        canvas.blend_jobs(L["blend"][0], L["blend"][1], None, out)
         if casts is not None:
             casts.after_blend(k, canvas, main)
         bufs[k] = None
-    if rest_done is not None:
-        main.wait_event(rest_done)
     if casts is not None:
         casts.join(main)
     # (every launch on the side streams is already joined through its event; a stream that never joined the capture must
@@ -751,23 +580,17 @@ class GraphedWaves:
         side.wait_stream(torch.cuda.current_stream(dp.device))
         saved = PROFILE
         PROFILE = None
-        # tile-granular DAG on several streams (no per-kernel profile, no tile dictionary: those stay wave mode)
-        self.dag = bool(order) and profile is None and not keep_processed and use_dag(dp.plan, order)
-        lanes = [torch.cuda.Stream(device=dp.device) for _ in range(max(dp.plan.dag(order)[0]) + 1)] if self.dag else []
-        self.split = (bool(order) and profile is None and not keep_processed and payload is None and not external_crop
+        # split crops only for the whole job as it is (no per-kernel profile, no tile dictionary, no payload, nothing skipped:
+        # bench.py's differencing and external_crop run the plain level loop)
+        self.split = (bool(order) and profile is None and not keep_processed and payload is None and not skip
                       and use_split(self.canvas, order))
-        if self.split:
-            lanes = [torch.cuda.Stream(device=dp.device), torch.cuda.Stream(device=dp.device)]
+        s_early = torch.cuda.Stream(device=dp.device) if self.split else None
         self.casts = None
-        if (casts and STREAM_OVERLAP and self.split and SCHEDULE == "split_crop" and not skip and canvas_buf is None
-                and CastBands.eligible(self.canvas)):
+        if casts and STREAM_OVERLAP and self.split and canvas_buf is None and CastBands.eligible(self.canvas):
             self.casts = CastBands(self.canvas, order, STREAM_BANDS, STREAM_CTAS)
 
         def body(warm_up=False):
-            if self.dag:
-                run_dag(self.canvas, order, denoiser, lanes, self.payload, where, skip)
-                return {}
-            if self.split and run_split(self.canvas, order, denoiser, lanes[0], lanes[1], skip, None if warm_up else self.casts):
+            if self.split and run_split(self.canvas, order, denoiser, s_early, None if warm_up else self.casts):
                 return {}
             if self.casts is not None:
                 raise nat.NativeError("canvas cast bands need the split schedule's job-record work lists")
@@ -810,7 +633,7 @@ class GraphedWaves:
         pkey = None if payload is None else (payload.data_ptr(), payload.numel())
         ckey = None if canvas_buf is None else canvas_buf.data_ptr()
         ckey_casts = (STREAM_OVERLAP, STREAM_CTAS, STREAM_BANDS, STREAM_PRIORITY) if casts else None
-        key = (id(dp), B, getattr(denoiser, "graph_key", id(denoiser)), id(profile), FORCE_GENERIC, FORCE_NO_MMA, SCHEDULE, FUSE_LEVELS,
+        key = (id(dp), B, getattr(denoiser, "graph_key", id(denoiser)), id(profile), FORCE_GENERIC, FORCE_NO_MMA, SCHEDULE,
                None if order is None else tuple(order), keep_processed, pkey, tuple(skip), ckey, external_crop, ckey_casts)
         return cls._cache.get_or_build(
             key, lambda: GraphedWaves(dp, B, denoiser, profile, order, keep_processed, payload, where, skip, canvas_buf,

@@ -5,7 +5,7 @@ The geometry, the table pool, the feather-mask specs, the tile descriptors, the 
 waves and the job records of the crop and blend kernels are built by libusdu_b200.so
 (csrc/usdu_plan.cpp, the planner section of include/usdu_b200.h), so that a host without
 Python drives the same plan; this module holds a plan handle and builds the schedules on top
-of those records: rank partitions, the tile-granular DAG, split and fused levels.
+of those records: rank partitions and split levels.
 
 Everything here is integer bookkeeping that the reference recomputes per tile with
 full-canvas PIL images; here it is computed once per job (and cached per geometry):
@@ -57,10 +57,6 @@ class Tile:
     @property
     def region(self) -> Tuple[int, int, int, int]:
         return (self.x1, self.y1, self.x2, self.y2)
-
-
-def _overlap(a: Tuple[int, int, int, int], b: Tuple[int, int, int, int]) -> bool:
-    return a[0] < b[2] and b[0] < a[2] and a[1] < b[3] and b[1] < a[3]
 
 
 # --------------------------------------------------------------------------------------
@@ -163,59 +159,6 @@ class Plan:
             out[lv].append(t)
         return out
 
-    # ---- tile-granular dependency graph ------------------------------------------------
-    def cover(self, t: Tile) -> Tuple[int, int, int, int]:
-        """Canvas rectangle a blend launch of tile t may LOAD AND STORE: its crop window grown to the block grid
-        of the kernels (128-px columns; rows for any block height up to FAST_BLOCK_H).  The blend kernels move
-        whole canvas blocks, so two tiles may run concurrently only if their covers are disjoint, not merely
-        their windows (a block shared by two concurrent launches would lose one of the two updates)."""
-        bw, bh = nat.FAST_BLOCK_W, nat.FAST_BLOCK_H
-        return (t.x1 // bw * bw, t.y1 - (bh - 1), (t.x2 + bw - 1) // bw * bw, t.y2 + (bh - 1))
-
-    MAX_LANES = 48
-
-    def dag(self, order: Optional[Sequence[int]] = None) -> Tuple[List[int], List[List[int]]]:
-        """The progressive job as a tile-granular DAG instead of level waves: tile k's chain (crop -> sampler ->
-        blend) may start as soon as the chains of the earlier tiles whose covers intersect its own are done --
-        which is all upscale/modes/single_gpu.py:40-64 requires, any topological order gives the same canvas.
-        -> (lane[i], waits[i]) for the i-th tile of `order`: the tile runs on stream `lane[i]` after the tiles at
-        positions `waits[i]` of other lanes (same-lane predecessors are ordered by the stream).  Lanes follow the
-        grid rows of a full canvas (tile (r, c) continues the lane of (r, c-1) and waits for (r-1, c+1)); tiles
-        without dependencies (a conflict-free partition) spread over up to MAX_LANES lanes."""
-        order = list(range(len(self.tiles))) if order is None else [int(t) for t in order]
-        pos = {t: i for i, t in enumerate(order)}
-        covers = {t: self.cover(self.tiles[t]) for t in order}
-        cell_w = max(c[2] - c[0] for c in covers.values()) if covers else 1
-        cell_h = max(c[3] - c[1] for c in covers.values()) if covers else 1
-        buckets: Dict[Tuple[int, int], List[int]] = {}
-        lane_of: List[int] = []
-        waits: List[List[int]] = []
-        tails: List[int] = []                       # position of the last tile queued on each lane
-        for i, t in enumerate(order):
-            c = covers[t]
-            cells = [(gx, gy) for gx in range(c[0] // cell_w, (c[2] - 1) // cell_w + 1)
-                     for gy in range(c[1] // cell_h, (c[3] - 1) // cell_h + 1)]
-            deps = sorted({pos[o] for cell in cells for o in buckets.get(cell, ()) if _overlap(covers[o], c)})
-            for cell in cells:
-                buckets.setdefault(cell, []).append(t)
-            dset = set(deps)
-            cand = [ln for ln, tail in enumerate(tails) if tail in dset]
-            if cand:
-                ln = max(cand, key=lambda q: tails[q])
-            elif len(tails) < self.MAX_LANES:
-                ln = len(tails)
-                tails.append(-1)
-            else:
-                ln = min(range(len(tails)), key=lambda q: tails[q])
-            latest: Dict[int, int] = {}
-            for d in deps:
-                if lane_of[d] != ln:
-                    latest[lane_of[d]] = max(latest.get(lane_of[d], -1), d)
-            lane_of.append(ln)
-            waits.append(sorted(latest.values()))
-            tails[ln] = i
-        return lane_of, waits
-
     def conflict_free(self, assignment: Sequence[Sequence[int]]) -> bool:
         for tiles in assignment:
             s = set(tiles)
@@ -291,11 +234,10 @@ class Plan:
                         rows=(int(info[nat.WL_ROW0]), int(info[nat.WL_ROW1])) if info[nat.WL_ROW0] >= 0 else None,
                         path=path, ks2=bool(info[nat.WL_KS2]))
 
-    def crop_worklist(self, tile_ids: Sequence[int], B: int, use_fast: Optional[bool] = None,
-                      share: int = 1) -> Tuple[WorkList, np.ndarray, int]:
+    def crop_worklist(self, tile_ids: Sequence[int], B: int, use_fast: Optional[bool] = None) -> Tuple[WorkList, np.ndarray, int]:
         """One crop launch over `tile_ids` (usdu_plan_crop_worklist) -> (work list, element offset of each tile's
         [B, ph, pw, 3] output in the packed buffer, total elements)."""
-        r = self._native.crop_worklist(tile_ids, B, self._request(use_fast), share, *self._launch_model())
+        r = self._native.crop_worklist(tile_ids, B, self._request(use_fast), *self._launch_model())
         return self._worklist(r, False), r["slots"], int(r["info"][nat.WL_TOTAL])
 
     def crop_split(self, wl: WorkList, prev_ids: Sequence[int]) -> np.ndarray:
@@ -322,27 +264,14 @@ class Plan:
         keep = int(mask.sum())
         return dataclasses.replace(wl, items=np.ascontiguousarray(J[mask]), algo_bytes=int(wl.algo_bytes * keep / max(J.shape[0], 1)))
 
-    def split_level(self, wave: Sequence[int], offs: np.ndarray, nxt: Optional[Sequence[int]], prev: Optional[Sequence[int]],
-                    B: int, path: int = 2):
+    def split_level(self, wave: Sequence[int], offs: np.ndarray, prev: Optional[Sequence[int]], B: int, path: int = 2):
         """Work lists of one dependency wave for the split schedule (engine.run_split).
-        -> (crop, offs, total, late mask or None, blend_crit, blend_rest or None).
+        -> (crop, offs, total, late mask or None, blend).
         crop jobs: `late` ones read pixels the previous wave `prev` changes, the rest may run beside the previous wave's
-        sampler and blends.  blend blocks: `crit` ones are read by a late crop job of the NEXT wave `nxt`, the rest only
-        has to land before the next wave's blends and the crops of the wave after it."""
+        sampler and blend."""
         cr, coffs, ctotal = self.crop_worklist(wave, B, path)
         late = self.crop_split(cr, prev) if (prev and cr.path >= 1) else None
-        if not nxt:
-            return cr, coffs, ctotal, late, self.blend_worklist(wave, offs, 4, path, B), None
-        ncr, _, _ = self.crop_worklist(nxt, B, path)
-        if ncr.path < 1:
-            return cr, coffs, ctotal, late, self.blend_worklist(wave, offs, 4, path, B), None
-        nl = self.crop_split(ncr, wave)
-        J = ncr.items.reshape(-1, nat.JOB_WORDS).astype(np.int64)[nl]
-        rects = np.stack([J[:, nat.J_SRC_A], J[:, nat.J_SRC_B], J[:, nat.J_SRC_A] + J[:, nat.J_COLS],
-                          J[:, nat.J_SRC_B] + J[:, nat.J_ROWS]], 1) if J.shape[0] else np.zeros((0, 4), np.int64)
-        crit = self.blend_worklist(wave, offs, 4, path, B, blocks=(rects, True))
-        rest = self.blend_worklist(wave, offs, 4, path, B, blocks=(rects, False))
-        return cr, coffs, ctotal, late, crit, rest
+        return cr, coffs, ctotal, late, self.blend_worklist(wave, offs, 4, path, B)
 
     CROP_BOX_ROWS = (0, 40, 48)           # rows of a crop's bulk-tensor box per kernel path (usdu_fast.cu / usdu_mma.cu kBoxR)
 
@@ -396,55 +325,14 @@ class Plan:
         return ([(y0, y1, int(first[y0:y1].min())) for y0, y1 in q],
                 [(y0, y1, int(last[y0:y1].max())) for y0, y1 in d])
 
-    MAX_LEVEL_DEPS = 4
-
-    def level_worklist(self, blend_ids: Sequence[int], offs: np.ndarray, crop_ids: Sequence[int], B: int, share: int = 1):
-        """Work lists of ONE launch that blends wave k (`blend_ids`, sampler output at element offsets `offs`) and crops
-        wave k+1 (`crop_ids`) with device-side ordering (usdu_level_blend_crop).  -> (blend WorkList, crop WorkList, crop
-        offsets, crop total elements, expect int32[n_slots]) or None when the plan / the launch does not qualify
-        (tensor-core records on both sides, crop patch inside the TMA boxes, at most MAX_LEVEL_DEPS dependencies per tile).
-        A crop tile depends on the tiles of `blend_ids` whose windows intersect its own (single_gpu.py:40-64: only
-        overlapping tiles are ordered); slots = positions in blend_ids."""
-        if self.kernel_path(None) != 2 or not blend_ids or not crop_ids:
-            return None
-        bl = self.blend_worklist(blend_ids, offs, 4, 2, B, None, share)
-        cr, coffs, ctotal = self.crop_worklist(crop_ids, B, 2, share)
-        if bl.path != 2 or cr.path != 2 or bl.n_launch <= 0 or (cr.patch_h & 0xFFFF) > 48 or 12 + cr.patch_w * 3 > 512:
-            return None
-        slot_of = {int(t): s for s, t in enumerate(blend_ids)}
-        J = cr.items.reshape(-1, nat.JOB_WORDS).copy()
-        dep_words = (nat.J_CX0, nat.J_CX1, nat.J_CY0, nat.J_FLAGS)
-        J[:, dep_words] = -1
-        tile_of_job = {}
-        row = 0
-        for tid in crop_ids:                       # crop records are laid out tile by tile, blocks row-major
-            t = self.tiles[tid]
-            n = len(range(0, t.pw, nat.FAST_BLOCK_W)) * len(range(0, t.ph, int(J[row, nat.J_CY1])))
-            deps = sorted(slot_of[n_] for n_ in self.neighbors[tid] if n_ in slot_of)
-            if len(deps) > self.MAX_LEVEL_DEPS:
-                return None
-            for d, w in zip(deps, dep_words):
-                J[row:row + n, w] = d
-            row += n
-        assert row == J.shape[0]
-        jb = bl.items.reshape(-1, nat.JOB_WORDS)
-        expect = np.bincount(jb[:, nat.J_SLOT], minlength=len(blend_ids)).astype(np.int32)
-        cr.items = np.ascontiguousarray(J)
-        return bl, cr, coffs, ctotal, expect
-
     def blend_worklist(self, tile_ids: Sequence[int], offs: np.ndarray, src_bytes_per_elem: int = 4,
-                       use_fast: Optional[bool] = None, B: int = 1, part: Optional[Tuple[int, int]] = None,
-                       share: int = 1, blocks: Optional[Tuple[np.ndarray, bool]] = None) -> WorkList:
+                       use_fast: Optional[bool] = None, B: int = 1, part: Optional[Tuple[int, int]] = None) -> WorkList:
         """Canvas blocks touched by the given tiles (usdu_plan_blend_worklist); each block lists its tiles in the
         given order (the order of `tile_ids` IS the blend order).  part = (i, n): only the blocks of the i-th of n
         horizontal slabs of the canvas (whole block rows, WorkList.rows = the slab's canvas rows; the n slabs tile
         the canvas) -- every block is owned by exactly one CTA, so n participants given the same tile list
-        composite disjoint slabs (dist.upscale_static: each rank finishes its own slab of the final canvas).
-        blocks = (rects int64 [m, 4] of canvas rectangles x0, y0, x1, y1, keep): only the blocks that intersect one of the
-        rectangles (keep = True) or none of them (keep = False) -- the two launches of a split level (split_level)."""
-        rects, keep = (None, -1) if blocks is None else (blocks[0], int(bool(blocks[1])))
-        r = self._native.blend_worklist(tile_ids, offs, src_bytes_per_elem, B, self._request(use_fast), part, share, rects, keep,
-                                        *self._launch_model())
+        composite disjoint slabs (dist.upscale_static: each rank finishes its own slab of the final canvas)."""
+        r = self._native.blend_worklist(tile_ids, offs, src_bytes_per_elem, B, self._request(use_fast), part, *self._launch_model())
         return self._worklist(r, True)
 
 

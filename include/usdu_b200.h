@@ -35,7 +35,7 @@ extern "C" {
 #pragma GCC visibility push(default) /* the library itself is built with -fvisibility=hidden */
 #endif
 
-#define USDU_ABI_VERSION 13
+#define USDU_ABI_VERSION 14
 
 typedef enum usdu_status {
     USDU_OK = 0,
@@ -136,7 +136,6 @@ typedef enum usdu_status {
 #define USDU_J_FRAME_LO 26 /* elements per frame PH*PW*3 */
 #define USDU_J_FRAME_HI 27
 #define USDU_J_NEXT 28     /* blend: index of the next record of the same block, -1 = last */
-#define USDU_J_SLOT 31     /* blend: position of the record's tile in the launch's tile list (usdu_level_blend_crop counts per tile) */
 #define USDU_J_TAPS_H 29   /* taps of the horizontal / vertical axis: 1..USDU_FAST_TAPS (packed rows of 8 int32; a value
                               <= 6 lets the kernel skip the unused last slot) or USDU_FAST_TAPS_WIDE (rows of 16) */
 #define USDU_J_TAPS_V 30
@@ -370,21 +369,6 @@ int usdu_tile_blend(uint8_t* canvas_dev, int B, int H, int W, int64_t pitch,
                     const int32_t* cover_dev, int patch_w, int patch_h, const void* src_dev,
                     int src_is_u8, int flags, void* stream);
 
-/* One launch per dependency level of the progressive job: the seam blend of wave k (bjobs: tensor-core blend records,
- * fp32 source = the sampler's output) AND the crop of wave k+1 (cjobs: tensor-core crop records) in one grid, ordered by
- * device-side ready counters instead of a kernel boundary: a crop block starts as soon as the tiles of wave k whose
- * windows touch its tile have been composited (its job words CX0, CX1, CY0, FLAGS = slots of those tiles in the blend
- * launch's tile list, -1 = none; expect_dev[slot] = canvas blocks that blend the tile).  sync_dev: 3 + n_slots * B
- * int32, zero before the first use (the kernel leaves it zero; word 2 is an error flag raised when a wait gives up).
- * Same results as usdu_tile_blend followed by usdu_tile_crop_resize (upscale/modes/single_gpu.py:40-64 only orders
- * OVERLAPPING tiles).  Tensor-core records only; the crop patch must fit the TMA boxes (USDU_ERR_UNSUPPORTED otherwise:
- * use the two separate launches). */
-int usdu_level_blend_crop(uint8_t* canvas_dev, int B, int H, int W, int64_t pitch, const int32_t* tabs_dev,
-                          const uint8_t* mask_pool_dev, const int32_t* bjobs_dev, int n_bheads, int b_patch_w,
-                          int b_patch_h, const float* src_dev, int block_rows, const int32_t* cjobs_dev,
-                          int n_cjobs, int c_patch_w, int c_patch_h, float* out_dev,
-                          const int32_t* expect_dev, int n_slots, int32_t* sync_dev, int flags, void* stream);
-
 /* ---- one-channel u8 planes: per-tile conditioning masks (utils/usdu_utils.py:415-442) ---------
  * Window of a separable 8bpc resize of n planes src[n][src_h][src_w] (Image.resize semantics:
  * horizontal pass first, u8 intermediate, then vertical): dst[p][j][i] = resized[p][oy+j][ox+i]
@@ -461,22 +445,19 @@ int usdu_plan_waves(const usdu_plan* plan, const int32_t* order, int n, int32_t*
 /* Work lists: one kernel launch each, built for
  *   path: 0 generic kernels, 1 integer-pipe (USDU_FLAG_FAST), 2 tensor-core (USDU_FLAG_MMA); lowered to what the plan
  *         supports (USDU_WL_PATH tells which);
- *   share: launches expected to run side by side (each gets 1/share of the machine in the block-height model);
  *   sm_count: SMs of the block-height model, 0 = query the current device (132 when there is none);
  *   mma_block_rows: tensor-core block height to force (16 or 32), 0 = the model's choice.
  * Crop: the tiles' [B][PH][PW][3] fp32 outputs are packed in list order (usdu_worklist_slots: element offset per tile,
  * USDU_WL_TOTAL elements in all).  Blend: src_offsets[i] = element offset of tile_ids[i]'s processed block in the
  * source, src_bytes = 4 (fp32) or 1 (u8); the list order is the blend order.  part_n > 0 restricts the launch to the
- * part_i-th of part_n horizontal slabs of canvas block rows (USDU_WL_ROW0 / _ROW1); select_keep = 1 / 0 keeps only the
- * canvas blocks that meet one / none of the n_rects rectangles {x0, y0, x1, y1} (int64), -1 = all blocks.
+ * part_i-th of part_n horizontal slabs of canvas block rows (USDU_WL_ROW0 / _ROW1).
  * Launch: items = usdu_worklist_items, grid = USDU_WL_GRID, flags = USDU_WL_FLAGS, patch = USDU_WL_PATCH_W / _H, and for
  * the generic blend cover_dev = usdu_worklist_cover. */
 typedef struct usdu_worklist usdu_worklist;
-int usdu_plan_crop_worklist(const usdu_plan* plan, const int32_t* tile_ids, int n, int B, int path, int share,
-                            int sm_count, int mma_block_rows, usdu_worklist** wl);
+int usdu_plan_crop_worklist(const usdu_plan* plan, const int32_t* tile_ids, int n, int B, int path, int sm_count,
+                            int mma_block_rows, usdu_worklist** wl);
 int usdu_plan_blend_worklist(const usdu_plan* plan, const int32_t* tile_ids, const int64_t* src_offsets, int n,
-                             int src_bytes, int B, int path, int part_i, int part_n, int share,
-                             const int64_t* select_rects, int n_rects, int select_keep, int sm_count,
+                             int src_bytes, int B, int path, int part_i, int part_n, int sm_count,
                              int mma_block_rows, usdu_worklist** wl);
 int usdu_worklist_destroy(usdu_worklist* wl);
 #define USDU_WL_INFO_WORDS 16      /* int64 words of usdu_worklist_info */

@@ -403,59 +403,6 @@ class Plan:
             out[lv].append(t)
         return out
 
-    # ---- tile-granular dependency graph ------------------------------------------------
-    def cover(self, t: Tile) -> Tuple[int, int, int, int]:
-        """Canvas rectangle a blend launch of tile t may LOAD AND STORE: its crop window grown to the block grid
-        of the kernels (128-px columns; rows for any block height up to FAST_BLOCK_H).  The blend kernels move
-        whole canvas blocks, so two tiles may run concurrently only if their covers are disjoint, not merely
-        their windows (a block shared by two concurrent launches would lose one of the two updates)."""
-        bw, bh = nat.FAST_BLOCK_W, nat.FAST_BLOCK_H
-        return (t.x1 // bw * bw, t.y1 - (bh - 1), (t.x2 + bw - 1) // bw * bw, t.y2 + (bh - 1))
-
-    MAX_LANES = 48
-
-    def dag(self, order: Optional[Sequence[int]] = None) -> Tuple[List[int], List[List[int]]]:
-        """The progressive job as a tile-granular DAG instead of level waves: tile k's chain (crop -> sampler ->
-        blend) may start as soon as the chains of the earlier tiles whose covers intersect its own are done --
-        which is all upscale/modes/single_gpu.py:40-64 requires, any topological order gives the same canvas.
-        -> (lane[i], waits[i]) for the i-th tile of `order`: the tile runs on stream `lane[i]` after the tiles at
-        positions `waits[i]` of other lanes (same-lane predecessors are ordered by the stream).  Lanes follow the
-        grid rows of a full canvas (tile (r, c) continues the lane of (r, c-1) and waits for (r-1, c+1)); tiles
-        without dependencies (a conflict-free partition) spread over up to MAX_LANES lanes."""
-        order = list(range(len(self.tiles))) if order is None else [int(t) for t in order]
-        pos = {t: i for i, t in enumerate(order)}
-        covers = {t: self.cover(self.tiles[t]) for t in order}
-        cell_w = max(c[2] - c[0] for c in covers.values()) if covers else 1
-        cell_h = max(c[3] - c[1] for c in covers.values()) if covers else 1
-        buckets: Dict[Tuple[int, int], List[int]] = {}
-        lane_of: List[int] = []
-        waits: List[List[int]] = []
-        tails: List[int] = []                       # position of the last tile queued on each lane
-        for i, t in enumerate(order):
-            c = covers[t]
-            cells = [(gx, gy) for gx in range(c[0] // cell_w, (c[2] - 1) // cell_w + 1)
-                     for gy in range(c[1] // cell_h, (c[3] - 1) // cell_h + 1)]
-            deps = sorted({pos[o] for cell in cells for o in buckets.get(cell, ()) if _overlap(covers[o], c)})
-            for cell in cells:
-                buckets.setdefault(cell, []).append(t)
-            dset = set(deps)
-            cand = [ln for ln, tail in enumerate(tails) if tail in dset]
-            if cand:
-                ln = max(cand, key=lambda q: tails[q])
-            elif len(tails) < self.MAX_LANES:
-                ln = len(tails)
-                tails.append(-1)
-            else:
-                ln = min(range(len(tails)), key=lambda q: tails[q])
-            latest: Dict[int, int] = {}
-            for d in deps:
-                if lane_of[d] != ln:
-                    latest[lane_of[d]] = max(latest.get(lane_of[d], -1), d)
-            lane_of.append(ln)
-            waits.append(sorted(latest.values()))
-            tails[ln] = i
-        return lane_of, waits
-
     def conflict_free(self, assignment: Sequence[Sequence[int]]) -> bool:
         for tiles in assignment:
             s = set(tiles)
@@ -517,13 +464,12 @@ class Plan:
         return (nat.sm_count() or cls.DEFAULT_SMS) * cls.CTAS_PER_SM
 
     def block_shape(self, use_fast: bool, extents: Optional[Sequence[Tuple[int, int]]] = None, frames: int = 1,
-                    share: int = 1, mma: bool = False) -> Tuple[int, int]:
+                    mma: bool = False) -> Tuple[int, int]:
         """Block edge of a launch.  `extents` = (width, height) in pixels each tile covers in
         the launch's block space.  The block height is chosen by a simple wave model:
         cost(bh) = ceil(#CTAs / resident slots) * (bh + halo/fixed rows) -- short blocks give
         small (latency bound) launches more CTAs, and large launches avoid a nearly empty
-        last wave.  share = launches expected to run side by side (tile-granular schedule): each gets
-        1/share of the machine."""
+        last wave."""
         if not use_fast:
             return self._generic_block
         bw = nat.FAST_BLOCK_W
@@ -534,7 +480,7 @@ class Plan:
         forced = os.environ.get("USDU_MMA_BH") if mma else None            # experiments: force the tensor-core block height
         for bh in (((int(forced),) if forced else (16, 32)) if mma else (8, 12, 16, 20, 24, 28, 32)):   # M-tiles are 16 output rows
             n = sum(((w + bw - 1) // bw + 1) * ((h + bh - 1) // bh + 1) for w, h in extents) * frames   # +1: unaligned windows
-            cost = math.ceil(n / max(slots // max(share, 1), 1)) * (bh + 12)
+            cost = math.ceil(n / max(slots, 1)) * (bh + 12)
             if best is None or cost < best[0] or (cost == best[0] and bh > best[1]):
                 best = (cost, bh)
         return bw, best[1]
@@ -590,15 +536,14 @@ class Plan:
                 return bh
         return 16
 
-    def crop_worklist(self, tile_ids: Sequence[int], B: int, use_fast: Optional[bool] = None,
-                      share: int = 1) -> Tuple[WorkList, np.ndarray, int]:
+    def crop_worklist(self, tile_ids: Sequence[int], B: int, use_fast: Optional[bool] = None) -> Tuple[WorkList, np.ndarray, int]:
         path = self.kernel_path(use_fast)
         use_fast = path >= 1
         offs, total = self.slot_offsets(tile_ids, B)
         rows = []
         pw_max = ph_max = 1
         nbytes = 0
-        bw, bh_max = self.block_shape(use_fast, [(self.tiles[t].pw - nat.FAST_BLOCK_W, self.tiles[t].ph) for t in tile_ids], B, share,
+        bw, bh_max = self.block_shape(use_fast, [(self.tiles[t].pw - nat.FAST_BLOCK_W, self.tiles[t].ph) for t in tile_ids], B,
                                       mma=path == 2)
         for i, tid in enumerate(tile_ids):
             t = self.tiles[tid]
@@ -648,63 +593,14 @@ class Plan:
         keep = int(mask.sum())
         return dataclasses.replace(wl, items=np.ascontiguousarray(J[mask]), algo_bytes=int(wl.algo_bytes * keep / max(J.shape[0], 1)))
 
-    def split_level(self, wave: Sequence[int], offs: np.ndarray, nxt: Optional[Sequence[int]], prev: Optional[Sequence[int]],
-                    B: int, path: int = 2):
+    def split_level(self, wave: Sequence[int], offs: np.ndarray, prev: Optional[Sequence[int]], B: int, path: int = 2):
         """Work lists of one dependency wave for the split schedule (engine.run_split).
-        -> (crop, offs, total, late mask or None, blend_crit, blend_rest or None).
+        -> (crop, offs, total, late mask or None, blend).
         crop jobs: `late` ones read pixels the previous wave `prev` changes, the rest may run beside the previous wave's
-        sampler and blends.  blend blocks: `crit` ones are read by a late crop job of the NEXT wave `nxt`, the rest only
-        has to land before the next wave's blends and the crops of the wave after it."""
+        sampler and blend."""
         cr, coffs, ctotal = self.crop_worklist(wave, B, path)
         late = self.crop_split(cr, prev) if (prev and cr.path >= 1) else None
-        if not nxt:
-            return cr, coffs, ctotal, late, self.blend_worklist(wave, offs, 4, path, B), None
-        ncr, _, _ = self.crop_worklist(nxt, B, path)
-        if ncr.path < 1:
-            return cr, coffs, ctotal, late, self.blend_worklist(wave, offs, 4, path, B), None
-        nl = self.crop_split(ncr, wave)
-        J = ncr.items.reshape(-1, nat.JOB_WORDS).astype(np.int64)[nl]
-        rects = np.stack([J[:, nat.J_SRC_A], J[:, nat.J_SRC_B], J[:, nat.J_SRC_A] + J[:, nat.J_COLS],
-                          J[:, nat.J_SRC_B] + J[:, nat.J_ROWS]], 1) if J.shape[0] else np.zeros((0, 4), np.int64)
-        crit = self.blend_worklist(wave, offs, 4, path, B, blocks=(rects, True))
-        rest = self.blend_worklist(wave, offs, 4, path, B, blocks=(rects, False))
-        return cr, coffs, ctotal, late, crit, rest
-
-    MAX_LEVEL_DEPS = 4
-
-    def level_worklist(self, blend_ids: Sequence[int], offs: np.ndarray, crop_ids: Sequence[int], B: int, share: int = 1):
-        """Work lists of ONE launch that blends wave k (`blend_ids`, sampler output at element offsets `offs`) and crops
-        wave k+1 (`crop_ids`) with device-side ordering (usdu_level_blend_crop).  -> (blend WorkList, crop WorkList, crop
-        offsets, crop total elements, expect int32[n_slots]) or None when the plan / the launch does not qualify
-        (tensor-core records on both sides, crop patch inside the TMA boxes, at most MAX_LEVEL_DEPS dependencies per tile).
-        A crop tile depends on the tiles of `blend_ids` whose windows intersect its own (single_gpu.py:40-64: only
-        overlapping tiles are ordered); slots = positions in blend_ids."""
-        if self.kernel_path(None) != 2 or not blend_ids or not crop_ids:
-            return None
-        bl = self.blend_worklist(blend_ids, offs, 4, 2, B, None, share)
-        cr, coffs, ctotal = self.crop_worklist(crop_ids, B, 2, share)
-        if bl.path != 2 or cr.path != 2 or bl.n_launch <= 0 or (cr.patch_h & 0xFFFF) > 48 or 12 + cr.patch_w * 3 > 512:
-            return None
-        slot_of = {int(t): s for s, t in enumerate(blend_ids)}
-        J = cr.items.reshape(-1, nat.JOB_WORDS).copy()
-        dep_words = (nat.J_CX0, nat.J_CX1, nat.J_CY0, nat.J_FLAGS)
-        J[:, dep_words] = -1
-        tile_of_job = {}
-        row = 0
-        for tid in crop_ids:                       # crop records are laid out tile by tile, blocks row-major
-            t = self.tiles[tid]
-            n = len(range(0, t.pw, nat.FAST_BLOCK_W)) * len(range(0, t.ph, int(J[row, nat.J_CY1])))
-            deps = sorted(slot_of[n_] for n_ in self.neighbors[tid] if n_ in slot_of)
-            if len(deps) > self.MAX_LEVEL_DEPS:
-                return None
-            for d, w in zip(deps, dep_words):
-                J[row:row + n, w] = d
-            row += n
-        assert row == J.shape[0]
-        jb = bl.items.reshape(-1, nat.JOB_WORDS)
-        expect = np.bincount(jb[:, nat.J_SLOT], minlength=len(blend_ids)).astype(np.int32)
-        cr.items = np.ascontiguousarray(J)
-        return bl, cr, coffs, ctotal, expect
+        return cr, coffs, ctotal, late, self.blend_worklist(wave, offs, 4, path, B)
 
     # ---- tensor-core job records ---------------------------------------------------------
     def _mma_axis(self, key: Tuple[int, int], base: np.ndarray, extent: np.ndarray):
@@ -813,22 +709,19 @@ class Plan:
         return J
 
     def blend_worklist(self, tile_ids: Sequence[int], offs: np.ndarray, src_bytes_per_elem: int = 4,
-                       use_fast: Optional[bool] = None, B: int = 1, part: Optional[Tuple[int, int]] = None,
-                       share: int = 1, blocks: Optional[Tuple[np.ndarray, bool]] = None) -> WorkList:
+                       use_fast: Optional[bool] = None, B: int = 1, part: Optional[Tuple[int, int]] = None) -> WorkList:
         """Canvas blocks touched by the given tiles; each block lists its tiles in the
         given order (the order of `tile_ids` IS the blend order).  part = (i, n): only the blocks of the i-th of n
         horizontal slabs of the canvas (whole block rows, WorkList.rows = the slab's canvas rows; the n slabs tile
         the canvas) -- every block is owned by exactly one CTA, so n participants given the same tile list
-        composite disjoint slabs (dist.upscale_static: each rank finishes its own slab of the final canvas).
-        blocks = (rects int64 [m, 4] of canvas rectangles x0, y0, x1, y1, keep): only the blocks that intersect one of the
-        rectangles (keep = True) or none of them (keep = False) -- the two launches of a split level (split_level)."""
+        composite disjoint slabs (dist.upscale_static: each rank finishes its own slab of the final canvas)."""
         path = self.kernel_path(use_fast)
         use_fast = path >= 1
         ext = []
         for t in tile_ids:
             sx0, sy0, sx1, sy1 = self.support(self.tiles[t])
             ext.append((sx1 - sx0, sy1 - sy0))
-        bw, bh = self.block_shape(use_fast, ext, B, share, mma=path == 2)
+        bw, bh = self.block_shape(use_fast, ext, B, mma=path == 2)
         nbx = (self.W + bw - 1) // bw
         nby = (self.H + bh - 1) // bh
         rows = None
@@ -836,14 +729,6 @@ class Plan:
             i, n = part
             lo_b, hi_b = (nby * i) // n, (nby * (i + 1)) // n
             rows = (min(lo_b * bh, self.H), min(hi_b * bh, self.H))
-        sel = None
-        if blocks is not None:
-            rects, keep = blocks
-            hit = np.zeros((nby, nbx), dtype=bool)
-            for rx0, ry0, rx1, ry1 in np.asarray(rects, dtype=np.int64).reshape(-1, 4).tolist():
-                if rx1 > rx0 and ry1 > ry0:
-                    hit[max(ry0, 0) // bh: (min(ry1, self.H) - 1) // bh + 1, max(rx0, 0) // bw: (min(rx1, self.W) - 1) // bw + 1] = True
-            sel = (hit if keep else ~hit).ravel()
         keys, tids, seq = [], [], []
         pw_max = ph_max = 1
         nbytes = 0
@@ -860,17 +745,12 @@ class Plan:
                 if gy.size == 0:
                     continue
             k = (gy[:, None] * nbx + gx[None, :]).ravel()
-            n_all = k.size
-            if sel is not None:
-                k = k[sel[k]]
-                if k.size == 0:
-                    continue
             keys.append(k)
             tids.append(np.full(k.size, tid, dtype=np.int64))
             seq.append(np.full(k.size, s, dtype=np.int64))
             pw_max = max(pw_max, self._span_max(t.pw, t.ew, bw, False))
             ph_max = max(ph_max, self._span_max(t.ph, t.eh, bh, False))
-            frac = (1.0 if part is None else gy.size * bh / max(Y1 - Y0, 1)) * (k.size / max(n_all, 1))
+            frac = 1.0 if part is None else gy.size * bh / max(Y1 - Y0, 1)
             nbytes += int(min(frac, 1.0) * (t.pw * t.ph * 3 * src_bytes_per_elem + 2 * (sx1 - sx0) * (sy1 - sy0) * 3))
         if not keys:
             return WorkList(np.zeros((0, nat.JOB_WORDS if use_fast else nat.BLEND_ITEM_WORDS), np.int32),
@@ -887,7 +767,7 @@ class Plan:
         items[:, 2] = first
         items[:, 3] = counts
         if use_fast:
-            jobs = self._blend_jobs(keys, tids, np.asarray(offs, dtype=np.int64)[seq], first, nbx, bw, bh, path == 2, seq)
+            jobs = self._blend_jobs(keys, tids, np.asarray(offs, dtype=np.int64)[seq], first, nbx, bw, bh, path == 2)
             if path == 2:
                 jobs, pw_max, ph_max = jobs
             ks2 = bool(path == 2 and (jobs[:, [nat.J_TAPS_H, nat.J_TAPS_V]] > 1).any())
@@ -901,7 +781,7 @@ class Plan:
                         block_rows=bh, block_cols=bw, rows=rows)
 
 
-    def _blend_jobs(self, keys, tids, src_off, first, nbx, bw, bh, mma: bool = False, seq=None):
+    def _blend_jobs(self, keys, tids, src_off, first, nbx, bw, bh, mma: bool = False):
         """(block, tile) pairs sorted by (block, blend order) -> fast job records; the first
         record of every block comes first (they form the grid), the rest is chained by NEXT.
         mma: tensor-core flavour of the records (-> records, patch_w, patch_h word)."""
@@ -966,8 +846,6 @@ class Plan:
         same = np.r_[keys[1:] == keys[:-1], False]
         nxt[same] = pos[1:][same[:-1]]
         J[:, nat.J_NEXT] = nxt
-        if seq is not None:
-            J[:, nat.J_SLOT] = seq                  # position of the record's tile in the launch's tile list
         out = np.zeros_like(J)
         out[pos] = J
         if mma:

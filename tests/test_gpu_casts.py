@@ -185,25 +185,22 @@ def _oracle_job(img, fn):
     return orc.process_single(img, fn, JOB["tile"], JOB["tile"], JOB["pad"], JOB["blur"], True)
 
 
-@pytest.mark.parametrize("schedule", ["split_crop", "waves", "fuse_levels"])
+@pytest.mark.parametrize("schedule", ["split_crop", "waves"])
 @pytest.mark.parametrize("out_dtype", [torch.float32, torch.float16])
 def test_job_with_an_out_of_range_sampler_and_image(family, schedule, out_dtype):
     """NaN, +-inf, +-1e10 and values just outside [0, 1] in the image (Q0) and in the sampler output (Q1), fp32 and
     fp16 sampler output; twice, so that the second call replays the captured wave graph."""
-    if schedule == "fuse_levels" and family != "mma":
-        pytest.skip("the fused level kernel is built for the tensor-core path only")
     img = _wild_image(1, JOB["H"], JOB["W"], 31)
     sampler = WildSampler(out_dtype)
     want = _oracle_job(img, sampler.numpy())
-    saved = engine.SCHEDULE, engine.FUSE_LEVELS
-    engine.SCHEDULE = "waves" if schedule == "waves" else "split_crop"
-    engine.FUSE_LEVELS = schedule == "fuse_levels"
+    saved = engine.SCHEDULE
+    engine.SCHEDULE = schedule
     try:
         for _ in range(2):
             got = _job(img, sampler).cpu().numpy()
             assert np.array_equal(got, want), f"{int((got != want).sum())} pixels differ from the oracle"
     finally:
-        engine.SCHEDULE, engine.FUSE_LEVELS = saved
+        engine.SCHEDULE = saved
 
 
 def _node_run(x, seed=5, den=0.5):

@@ -71,32 +71,13 @@ def test_node_api_on_a_host_tensor_matches_the_reference_digest(name):
         del out
 
 
-def test_fused_level_launches_give_the_same_canvas():
-    """engine.FUSE_LEVELS: blend(k) U crop(k+1) as one launch ordered by device-side ready counters
-    (usdu_level_blend_crop) -- off by default (not faster than the level loop), kept correct: same digest as the reference on cfg2."""
-    B, H, W, tile, pad, blur = WORKLOADS["cfg2_4k_to_8k_sdxl_512px"]
-    want = _expected("cfg2_4k_to_8k_sdxl_512px")
-    img = _canvas(B, H, W).cuda()
-    engine.FUSE_LEVELS = True
-    try:
-        for _ in range(3):                   # eager warm-up inside the capture, then replays: the counters must return to zero
-            out = engine.upscale_single(img, T0Denoiser(321, 0.5), tile, tile, pad, blur, True)
-            del out
-        out = engine.upscale_single(img, T0Denoiser(123, 0.5), tile, tile, pad, blur, True)
-        assert _digest(out) == want
-    finally:
-        engine.FUSE_LEVELS = False
-
-
-@pytest.mark.parametrize("name,schedule", [("cfg2_4k_to_8k_sdxl_512px", "split_crop"), ("cfg2_4k_to_8k_sdxl_512px", "split"),
-                                           ("cfg2_4k_to_8k_sdxl_512px", "split_blend"), ("cfg2_4k_to_8k_sdxl_512px", "split_crop_a"),
-                                           ("cfg2_4k_to_8k_sdxl_512px", "waves"), ("cfg5_video_17f_4k", "split"),
-                                           ("cfg5_video_17f_4k", "waves"), ("cfg1_512_256px", "split")])
+@pytest.mark.parametrize("name,schedule", [("cfg2_4k_to_8k_sdxl_512px", "split_crop"), ("cfg2_4k_to_8k_sdxl_512px", "waves"),
+                                           ("cfg5_video_17f_4k", "split_crop"), ("cfg5_video_17f_4k", "waves"),
+                                           ("cfg1_512_256px", "split_crop")])
 def test_every_level_schedule_gives_the_same_canvas(name, schedule):
     """engine.SCHEDULE: "split_crop" is the default (engine.run_split: the crop jobs of wave k+1 that do not read what wave
-    k changes run on a second stream beside sampler(k) / blend(k)); "split" also splits the blends (crit / rest, three
-    streams), "split_blend" only those, "split_crop_a" forks the early crops one step earlier, "waves" is the plain level
-    loop -- the same digest as the reference on every replay of every one of them."""
+    k changes run on a second stream beside sampler(k) / blend(k)); "waves" is the plain level loop -- the same digest as
+    the reference on every replay of both."""
     B, H, W, tile, pad, blur = WORKLOADS[name]
     want = _expected(name)
     img = _canvas(B, H, W).cuda()
@@ -109,6 +90,6 @@ def test_every_level_schedule_gives_the_same_canvas(name, schedule):
             del out
         if name != "cfg1_512_256px":                    # (cfg1 has 4 single-tile waves: run_split has nothing to split)
             gw = list(engine.GraphedWaves._cache.values())[-1]
-            assert gw.split == schedule.startswith("split")
+            assert gw.split == (schedule == "split_crop")
     finally:
         engine.SCHEDULE = saved

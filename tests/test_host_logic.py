@@ -362,38 +362,6 @@ def test_table_builders_fuzz_against_oracle():
         assert np.array_equal(nat.nearest_index(n_in, n_out), orc.nearest_index(n_in, n_out))
 
 
-@pytest.mark.parametrize("W,H,tile,pad", [(7680, 4320, 512, 32), (1300, 1100, 256, 32), (1000, 900, 256, 64), (640, 640, 500, 24)])
-def test_tile_dag_is_a_valid_parallel_schedule_of_the_progressive_order(W, H, tile, pad):
-    """Plan.dag (engine.run_dag): every pair of tiles whose block covers intersect is ordered -- by the lane (stream) they
-    share or through a chain of waits -- in the direction of the progressive order; waits point backwards; the depth of the
-    DAG equals the number of level waves."""
-    p = planner.Plan.build(W, H, tile, tile, pad, 8, True)
-    order = list(range(len(p.tiles)))
-    lanes, waits = p.dag(order)
-    n = len(order)
-    assert len(lanes) == len(waits) == n and max(lanes) + 1 <= p.MAX_LANES
-    pred = [set() for _ in range(n)]            # transitive predecessors through lanes and waits
-    last = {}
-    depth = [0] * n
-    for i in range(n):
-        direct = set(waits[i])
-        assert all(w < i and lanes[w] != lanes[i] for w in direct)
-        if lanes[i] in last:
-            direct.add(last[lanes[i]])
-        last[lanes[i]] = i
-        for d in direct:
-            pred[i] |= pred[d] | {d}
-            depth[i] = max(depth[i], depth[d] + 1)
-    covers = [p.cover(p.tiles[t]) for t in order]
-    for i in range(n):
-        for j in range(i):
-            a, b = covers[i], covers[j]
-            if a[0] < b[2] and b[0] < a[2] and a[1] < b[3] and b[1] < a[3]:
-                assert j in pred[i], (i, j)
-    assert max(depth) + 1 >= len(p.waves())     # never shallower than the true dependency depth ...
-    assert max(depth) + 1 <= len(p.waves()) + 2  # ... and no long false chains
-
-
 def test_caches_evict_the_least_recently_used_entry_only():
     """Alternating geometries keep their plans (and, on the device, tables and graphs) warm: the host caches are LRU,
     they never drop everything at once."""

@@ -121,15 +121,14 @@ def test_library_plan_equals_the_numpy_model(case, launch_model):
     for path in (0, 1, 2):
         lists = [list(range(T))] + [sorted(w, key=lambda t: (m.tiles[t].ph, m.tiles[t].pw, t)) for w in waves[:2 if big else 4]]
         for k, ids in enumerate(lists):
-            share = 1 + (k + i) % 3
-            got, goffs, gtotal = p.crop_worklist(ids, B, path, share)
-            want, woffs, wtotal = m.crop_worklist(ids, B, path, share)
+            got, goffs, gtotal = p.crop_worklist(ids, B, path)
+            want, woffs, wtotal = m.crop_worklist(ids, B, path)
             _same_worklist(got, want, (name, "crop", path, k))
             assert np.array_equal(goffs, woffs) and gtotal == wtotal
             offs = woffs + (0 if k % 2 else (5 << 32) + 48)            # source offsets beyond 2^32
             for src_bytes in (4, 1):
-                _same_worklist(p.blend_worklist(ids, offs, src_bytes, path, B, None, share),
-                               m.blend_worklist(ids, offs, src_bytes, path, B, None, share), (name, "blend", path, k, src_bytes))
+                _same_worklist(p.blend_worklist(ids, offs, src_bytes, path, B),
+                               m.blend_worklist(ids, offs, src_bytes, path, B), (name, "blend", path, k, src_bytes))
             if k == 0 or not big:
                 n = 2 + (i + k) % 3
                 for part_i in range(n):
@@ -139,9 +138,9 @@ def test_library_plan_equals_the_numpy_model(case, launch_model):
 
 @pytest.mark.parametrize("case", [c for c in CASES if c[0] in ("cfg1", "cfg2", "blur255_pad256", "w_not_mult4", "nonuniform_odd_w")],
                          ids=lambda c: c[0])
-def test_split_and_fused_level_lists_equal_the_numpy_model(case, launch_model):
-    """The schedules that stay in Python consume the library's records: split levels (blend lists restricted to the
-    blocks some rectangles meet, or to the others) and fused levels."""
+def test_split_level_lists_equal_the_numpy_model(case, launch_model):
+    """The split schedule, which stays in Python, consumes the library's records: per wave the crop list, the mask of its
+    late jobs and the blend list."""
     name, W, H, tw, th, pad, blur, uniform, B = case
     launch_model(132)
     p, m = planner.Plan.build(W, H, tw, th, pad, blur, uniform), pm.Plan.build(W, H, tw, th, pad, blur, uniform)
@@ -149,30 +148,12 @@ def test_split_and_fused_level_lists_equal_the_numpy_model(case, launch_model):
     for path in (1, 2):
         for k, w in enumerate(waves):
             offs, _ = m.slot_offsets(w, B)
-            nxt = waves[k + 1] if k + 1 < len(waves) else None
             prev = waves[k - 1] if k else None
-            got, want = p.split_level(w, offs, nxt, prev, B, path), m.split_level(w, offs, nxt, prev, B, path)
+            got, want = p.split_level(w, offs, prev, B, path), m.split_level(w, offs, prev, B, path)
             _same_worklist(got[0], want[0], (name, "split crop", k))
             assert np.array_equal(got[1], want[1]) and got[2] == want[2]
             assert (got[3] is None) == (want[3] is None) and (got[3] is None or np.array_equal(got[3], want[3]))
-            for g, wl in zip(got[4:], want[4:]):
-                assert (g is None) == (wl is None)
-                if wl is not None:
-                    _same_worklist(g, wl, (name, "split blend", k))
-            if nxt:
-                got, want = p.level_worklist(w, offs, nxt, B), m.level_worklist(w, offs, nxt, B)
-                assert (got is None) == (want is None)
-                if want is not None:
-                    for g, wl in zip(got[:2], want[:2]):
-                        _same_worklist(g, wl, (name, "level", k))
-                    assert np.array_equal(got[2], want[2]) and got[3] == want[3] and np.array_equal(got[4], want[4])
-    rects = np.array([[0, 0, W // 3, H // 2], [W // 2, H // 3, W + 50, H + 50], [-40, -40, 10, 10]], np.int64)
-    ids = list(range(len(p.tiles)))
-    offs, _ = m.slot_offsets(ids, B)
-    for path in (0, 1, 2):
-        for keep in (True, False):
-            _same_worklist(p.blend_worklist(ids, offs, 4, path, B, blocks=(rects, keep)),
-                           m.blend_worklist(ids, offs, 4, path, B, blocks=(rects, keep)), (name, "blocks", path, keep))
+            _same_worklist(got[4], want[4], (name, "split blend", k))
 
 
 def test_empty_lists_and_the_default_launch_model(monkeypatch):

@@ -194,54 +194,16 @@ def test_generic_work_items_cover_every_output_once_and_fit_the_declared_patch(W
             assert (int(cover[j, 1]) & 0xFFFFFFFF) | (int(cover[j, 2]) << 32) == boffs[int(cover[j, 0])]
 
 
-@pytest.mark.parametrize("W,H,tile,pad,blur", [(1600, 1200, 512, 32, 8), (2048, 1536, 256, 32, 16), (7680, 4320, 512, 32, 8)])
-def test_level_worklists_order_every_crop_after_the_blends_it_reads(W, H, tile, pad, blur):
-    """usdu_level_blend_crop runs blend(wave k) and crop(wave k+1) in one grid; the planner's part is the dependency
-    slots of the crop records and the per-tile block counts.  For every pair of consecutive waves: a crop job names every
-    tile of wave k whose feather support intersects the canvas rectangle the job stages, and expect[slot] equals the
-    number of block chains that contain the tile (so the counters reach it exactly when the tile is fully composited)."""
-    p = planner.Plan.build(W, H, tile, tile, pad, blur, True)
-    if not p.mma:
-        pytest.skip("no tensor-core path")
-    waves = p.waves()
-    checked = 0
-    for k in range(len(waves) - 1):
-        offs, _ = p.slot_offsets(waves[k], 1)
-        r = p.level_worklist(waves[k], offs, waves[k + 1], 1)
-        assert r is not None
-        bl, cr, coffs, ctotal, expect = r
-        jb = bl.items.reshape(-1, nat.JOB_WORDS)
-        chains = np.zeros(len(waves[k]), dtype=np.int64)
-        for h in range(bl.n_launch):
-            i = h
-            while i >= 0:
-                chains[jb[i, nat.J_SLOT]] += 1
-                i = int(jb[i, nat.J_NEXT])
-        assert np.array_equal(chains, expect) and chains.sum() == jb.shape[0]
-        for J in cr.items.reshape(-1, nat.JOB_WORDS):
-            x0, y0 = int(J[nat.J_SRC_A]), int(J[nat.J_SRC_B])
-            rect = (x0, y0, x0 + int(J[nat.J_COLS]), y0 + int(J[nat.J_ROWS]))
-            deps = {int(J[w]) for w in (nat.J_CX0, nat.J_CX1, nat.J_CY0, nat.J_FLAGS) if J[w] >= 0}
-            for s, tid in enumerate(waves[k]):
-                t = p.tiles[tid]
-                sx0, sy0, sx1, sy1 = p.support(t)
-                sup = (t.x1 + sx0, t.y1 + sy0, t.x1 + sx1, t.y1 + sy1)
-                if sup[0] < rect[2] and rect[0] < sup[2] and sup[1] < rect[3] and rect[1] < sup[3]:
-                    assert s in deps, (k, tid, rect, sup)
-                    checked += 1
-    assert checked > 0
-
-
 @pytest.mark.parametrize("W,H,tile,pad,blur,B,extreme,path", [
-    (1100, 900, 256, 32, 16, 1, "rest_last_early_first", 2), (700, 560, 128, 16, 8, 2, "rest_last_early_first", 2),
-    (700, 560, 128, 16, 8, 2, "rest_first_early_last", 2), (640, 512, 128, 16, 8, 1, "rest_last_early_first", 1)])
+    (1100, 900, 256, 32, 16, 1, "early_first", 2), (700, 560, 128, 16, 8, 2, "early_first", 2),
+    (700, 560, 128, 16, 8, 2, "early_last", 2), (640, 512, 128, 16, 8, 1, "early_first", 1)])
 #   (2300 x 1500 / 512, both orders: checked once, 3 min)
 def test_split_levels_give_the_sequential_result_in_every_legal_order(W, H, tile, pad, blur, B, extreme, path):
-    """engine.run_split launches, per dependency wave, crop_early / crop_late and blend_crit / blend_rest
-    (planner.split_level) on three streams.  The numpy model executes the same lists SEQUENTIALLY in the two extreme
-    interleavings the stream dependencies allow -- the early crops of wave k+1 before ANY blend of wave k and
-    blend_rest(k) after the sampler of wave k+1, or the other way round -- and must reproduce the oracle's
-    process_single (tile after tile) bit for bit: the split only reorders work that does not interact."""
+    """engine.run_split launches, per dependency wave, crop_early / crop_late and one blend (planner.split_level) on two
+    streams.  The numpy model executes the same lists SEQUENTIALLY in the two extreme placements the stream dependencies
+    allow the early crops of wave k+1 -- before ANY blend of wave k, or right before the sampler of wave k+1 needs them --
+    and must reproduce the oracle's process_single (tile after tile) bit for bit: the split only reorders work that does
+    not interact."""
     p = planner.Plan.build(W, H, tile, tile, pad, blur, True)
     if not (p.mma if path == 2 else p.fast):
         pytest.skip("no job-record path")
@@ -257,17 +219,13 @@ def test_split_levels_give_the_sequential_result_in_every_legal_order(W, H, tile
     L = []
     for k, w in enumerate(waves):
         offs, _ = p.slot_offsets(w, B)
-        cr, coffs, ctotal, late, crit, rest = p.split_level(w, offs, waves[k + 1] if k + 1 < len(waves) else None,
-                                                            waves[k - 1] if k else None, B, path)
+        cr, coffs, ctotal, late, blend = p.split_level(w, offs, waves[k - 1] if k else None, B, path)
         assert np.array_equal(coffs, offs)
         early = lt = None
         if late is not None and late.any() and not late.all():
             early, lt = p.sub_worklist(cr, ~late), p.sub_worklist(cr, late)
-        if rest is not None:                                     # the two blend launches share out the blocks of the wave
-            full = p.blend_worklist(w, offs, 4, path, B)
-            assert crit.n_launch + rest.n_launch == full.n_launch and crit.block_rows == rest.block_rows == full.block_rows
-        L.append(dict(crop=cr, early=early, late=lt, total=ctotal, offs=offs, crit=crit, rest=rest))
-    assert any(e["early"] is not None for e in L) and any(e["rest"] is not None and e["rest"].n_launch > 0 for e in L)
+        L.append(dict(crop=cr, early=early, late=lt, total=ctotal, offs=offs, blend=blend))
+    assert any(e["early"] is not None for e in L)
 
     def sample(k, buf):
         out = np.empty_like(buf)
@@ -278,7 +236,6 @@ def test_split_levels_give_the_sequential_result_in_every_legal_order(W, H, tile
         return out
 
     bufs = {0: np.full(L[0]["total"], -1.0, np.float32)}
-    pending_rest = None                                           # (work list, sampler output) of blend_rest(k-1)
     early_pending = {}
     for k in range(len(waves)):
         e = L[k]
@@ -290,23 +247,13 @@ def test_split_levels_give_the_sequential_result_in_every_legal_order(W, H, tile
             run_crop(p, canvas, e["crop"], bufs[k])
         assert not (bufs[k] < 0).any()
         out = sample(k, bufs[k])
-        this_rest = (e["rest"], out) if e["rest"] is not None and e["rest"].n_launch > 0 else None
-        if extreme == "rest_first_early_last" and this_rest is not None:
-            run_blend(p, canvas, this_rest[0], this_rest[1], pool)
-            this_rest = None
-        if pending_rest is not None:                              # the join: blend_rest(k-1) at the latest here
-            run_blend(p, canvas, pending_rest[0], pending_rest[1], pool)
-        pending_rest = this_rest
         if k + 1 < len(waves):
             bufs[k + 1] = np.full(L[k + 1]["total"], -1.0, np.float32)
             if L[k + 1]["early"] is not None:
-                if extreme == "rest_last_early_first":            # before any blend of wave k
+                if extreme == "early_first":                      # before any blend of wave k
                     run_crop(p, canvas, L[k + 1]["early"], bufs[k + 1])
                 else:
                     early_pending[k + 1] = L[k + 1]["early"]
-        if e["crit"].n_launch != 0:
-            run_blend(p, canvas, e["crit"], out, pool)
+        run_blend(p, canvas, e["blend"], out, pool)
         del bufs[k]
-    if pending_rest is not None:
-        run_blend(p, canvas, pending_rest[0], pending_rest[1], pool)
     assert np.array_equal(orc.dequantize_u8(canvas), want)
