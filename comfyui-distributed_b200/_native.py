@@ -16,7 +16,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libusdu_b200.so")
 
 # constants mirrored from include/usdu_b200.h (checked against the header in tests)
-ABI_VERSION = 14
+ABI_VERSION = 15
 ERR_INVALID = -1
 CANVAS_SLACK = 16
 PLAN_INFO_WORDS = 16
@@ -122,6 +122,9 @@ _SIGNATURES = {
     "usdu_plan_crop_worklist": (c_int, [c_void_p, POINTER(c_int32), c_int, c_int, c_int, c_int, c_int, POINTER(c_void_p)]),
     "usdu_plan_blend_worklist": (c_int, [c_void_p, POINTER(c_int32), POINTER(c_int64), c_int, c_int, c_int, c_int, c_int,
                                          c_int, c_int, c_int, POINTER(c_void_p)]),
+    "usdu_plan_split_worklists": (c_int, [c_void_p, POINTER(c_int32), POINTER(c_int64), c_int, POINTER(c_int32), c_int, c_int,
+                                          c_int, c_int, POINTER(c_void_p), POINTER(c_void_p), POINTER(c_void_p)]),
+    "usdu_mma_resident_ctas": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int]),
     "usdu_worklist_destroy": (c_int, [c_void_p]),
     "usdu_worklist_info": (c_int, [c_void_p, POINTER(c_int64)]),
     "usdu_worklist_items": (c_int, [c_void_p, POINTER(c_int32)]),
@@ -168,6 +171,18 @@ def _check(status: int, what: str):
 def _i32p(a: np.ndarray):
     assert a.dtype == np.int32 and a.flags["C_CONTIGUOUS"]
     return a.ctypes.data_as(POINTER(c_int32))
+
+
+KERNEL_CROP_LDG, KERNEL_CROP_TMA, KERNEL_BLEND, KERNEL_LARGE = 0, 1, 2, 4
+
+
+def resident_ctas(kernel: int, two_ksteps: bool, patch_w: int, patch_h: int, block_rows: int, use_device: bool) -> int:
+    """Resident CTAs per SM of a tensor-core kernel build at the shared memory its launcher requests for these patch
+    words (usdu_mma_resident_ctas): the device's occupancy calculator, or the library's table without it."""
+    n = lib().usdu_mma_resident_ctas(kernel, int(two_ksteps), patch_w, patch_h, block_rows, int(use_device))
+    if n < 0:
+        _check(n, "usdu_mma_resident_ctas")
+    return n
 
 
 # ---- host-side builders -------------------------------------------------------------
@@ -333,6 +348,28 @@ class NativePlan:
         out = _read_worklist(h)
         out["slots"] = slots[:ids.size]
         return out
+
+    def split_worklists(self, tile_ids, offs, prev_ids, B: int, path: int, sm_count: int) -> tuple:
+        """-> (late crop, early crop, blend) of one wave of the split schedule; the crops carry "slots"."""
+        ids, prev = _ids(tile_ids), _ids(prev_ids)
+        offs = np.ascontiguousarray(np.asarray(offs, dtype=np.int64).reshape(-1))
+        if offs.size < ids.size:
+            raise ValueError(f"split work lists: {offs.size} source offsets for {ids.size} tiles")
+        offs = np.ascontiguousarray(offs[:max(ids.size, 1)]) if offs.size else np.zeros(1, np.int64)
+        hs = [c_void_p() for _ in range(3)]
+        _check(self._lib.usdu_plan_split_worklists(self._h, _i32p(ids), _i64p(offs), ids.size, _i32p(prev), prev.size, B, path,
+                                                   sm_count, *[ctypes.byref(h) for h in hs]), "usdu_plan_split_worklists")
+        slots = np.zeros(max(ids.size, 1), np.int64)
+        try:
+            if ids.size:
+                _check(self._lib.usdu_worklist_slots(hs[0], _i64p(slots)), "usdu_worklist_slots")
+        except BaseException:
+            for h in hs:
+                self._lib.usdu_worklist_destroy(h)
+            raise
+        out = [_read_worklist(h) for h in hs]
+        out[0]["slots"] = out[1]["slots"] = slots[:ids.size]
+        return tuple(out)
 
     def blend_worklist(self, tile_ids, offs, src_bytes: int, B: int, path: int, part, sm_count: int, mma_block_rows: int) -> dict:
         """part = (i, n) or None."""

@@ -670,5 +670,50 @@ int launch_blend(uint8_t* canvas, int B, int H, int W, int64_t pitch, const int3
                       : launch_one(blend_mma_kernel<false, 1>, smem, grid, st, tabs, mask_pool, items, src, W3, patch_w, plane_rows, mid_rows, block_rows, cmap);
 }
 
+// Resident CTAs per SM of the build launch_crop / launch_blend would pick (kernel = USDU_KERNEL_*, the crop's
+// USDU_KERNEL_LARGE bit as kLargeGridPerSM decides it) at the dynamic shared memory it would request for these patch
+// words.  use_device: cudaOccupancyMaxActiveBlocksPerMultiprocessor on the current device; else the table of the
+// launch bounds (kOccSmall / kOccLarge, which ptxas meets: 80 / 64 registers at most) and 228 KB of shared memory per
+// SM, 1 KB of it reserved per CTA.  0 when the build does not fit an SM, a negative usdu_status on an error.
+int resident_ctas(int kernel, bool two_ksteps, int patch_w, int patch_h, int block_rows, bool use_device) {
+    const int plane_rows = patch_h & 0xFFFF, mid_rows = (patch_h >> 16) & 0xFFFF;
+    const int base = kernel & ~USDU_KERNEL_LARGE;
+    const bool large = (kernel & USDU_KERNEL_LARGE) && base != USDU_KERNEL_BLEND && !two_ksteps;
+    size_t smem;
+    const void* fn;
+    if (base == USDU_KERNEL_BLEND) {
+        smem = blend_smem(patch_w, plane_rows, mid_rows, block_rows);
+        fn = two_ksteps ? (const void*)blend_mma_kernel<false, 2> : (const void*)blend_mma_kernel<false, 1>;
+    } else if (base == USDU_KERNEL_CROP_LDG || base == USDU_KERNEL_CROP_TMA) {
+        const bool tma = base == USDU_KERNEL_CROP_TMA;
+        smem = crop_smem(patch_w, plane_rows, mid_rows, tma);
+        fn = two_ksteps ? (tma ? (const void*)crop_mma_kernel<1, 2, kOccSmall> : (const void*)crop_mma_kernel<0, 2, kOccSmall>)
+             : large    ? (tma ? (const void*)crop_mma_kernel<1, 1, kOccLarge> : (const void*)crop_mma_kernel<0, 1, kOccLarge>)
+                        : (tma ? (const void*)crop_mma_kernel<1, 1, kOccSmall> : (const void*)crop_mma_kernel<0, 1, kOccSmall>);
+    } else {
+        set_error("usdu_mma_resident_ctas: unknown kernel %d", kernel);
+        return USDU_ERR_INVALID;
+    }
+    if (smem > 227 * 1024) return 0;
+    if (!use_device) {
+        const size_t per_cta = (smem + 1024 + 127) / 128 * 128;
+        return (int)std::min((size_t)(large ? kOccLarge : kOccSmall), (size_t)228 * 1024 / per_cta);
+    }
+    int s = raise_smem_limit(fn, smem);
+    if (s != USDU_OK) return s;
+    int n = 0;
+    USDU_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, fn, kT, smem));
+    return n;
+}
+
 }  // namespace mma
 }  // namespace usdu
+
+int usdu_mma_resident_ctas(int kernel, int two_ksteps, int patch_w, int patch_h, int block_rows, int use_device) {
+    if (patch_w <= 0 || (patch_h & 0xFFFF) <= 0 || ((patch_h >> 16) & 0xFFFF) < (patch_h & 0xFFFF) || block_rows < 0 ||
+        block_rows > USDU_FAST_BLOCK_H) {
+        usdu::set_error("usdu_mma_resident_ctas: bad patch (w=%d h=%#x) or block height %d", patch_w, patch_h, block_rows);
+        return USDU_ERR_INVALID;
+    }
+    return usdu::mma::resident_ctas(kernel, two_ksteps != 0, patch_w, patch_h, block_rows, use_device != 0);
+}

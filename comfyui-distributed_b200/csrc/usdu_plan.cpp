@@ -26,6 +26,9 @@
 namespace usdu {
 void set_error(const char* fmt, ...);
 int sm_count();
+namespace mma {
+int resident_ctas(int kernel, bool two_ksteps, int patch_w, int patch_h, int block_rows, bool use_device);
+}
 }  // namespace usdu
 
 namespace {
@@ -852,6 +855,122 @@ int blend_worklist(Plan* p, const int32_t* ids, const int64_t* offs, int n, int 
     return USDU_OK;
 }
 
+// Does job record r stage a canvas pixel that the blend of a tile in prev[0..n_prev) changes (its feather support)?
+bool meets(const Plan* p, const int32_t* r, const int32_t* prev, int n_prev) {
+    const int64_t x0 = r[USDU_J_SRC_A], y0 = r[USDU_J_SRC_B];
+    const int64_t x1 = x0 + r[USDU_J_LEAD] + r[USDU_J_COLS], y1 = y0 + r[USDU_J_ROWS];   // (integer-pipe records start `lead` pixels early)
+    for (int i = 0; i < n_prev; ++i) {
+        const Tile& t = p->tiles[prev[i]];
+        int64_t s[4];
+        p->support(t, s);
+        if (s[2] > s[0] && s[3] > s[1] && x0 < t.x1 + s[2] && t.x1 + s[0] < x1 && y0 < t.y1 + s[3] && t.y1 + s[1] < y1) return true;
+    }
+    return false;
+}
+
+int64_t job_outputs(const int32_t* r) { return (int64_t)r[USDU_J_ROWS_OUT] * r[USDU_J_COLS_OUT]; }
+
+// The jobs `pick` of crop lists (each entry: list, record index) as one launch: the layout of `shape`, patch words that
+// hold every job's staging, algorithmic bytes by share of the outputs.
+void take_jobs(const std::vector<std::pair<const WorkList*, size_t>>& pick, const WorkList& shape, int64_t all_outputs,
+               WorkList* wl) {
+    *wl = shape;
+    wl->items.clear();
+    int64_t outputs = 0, plane = shape.patch_h & 0xFFFF, mid = shape.patch_h >> 16;
+    for (const auto& q : pick) {
+        const int32_t* r = q.first->items.data() + q.second * USDU_JOB_WORDS;
+        wl->items.insert(wl->items.end(), r, r + USDU_JOB_WORDS);
+        outputs += job_outputs(r);
+        wl->patch_w = std::max(wl->patch_w, q.first->patch_w);
+        plane = std::max(plane, q.first->patch_h & 0xFFFF);
+        mid = std::max(mid, q.first->patch_h >> 16);
+    }
+    if (shape.path == 2) wl->patch_h = plane | (mid << 16);
+    wl->algo_bytes = (int64_t)((double)shape.algo_bytes * (double)outputs / (double)std::max(all_outputs, (int64_t)1));
+    wl->ks2 = shape.path == 2 && any_ks2(wl->items);
+}
+
+int split_worklists(Plan* p, const int32_t* ids, const int64_t* offs, int n, const int32_t* prev, int n_prev, int B,
+                    int req_path, const LaunchModel& m, WorkList* late, WorkList* early, WorkList* blend) {
+    const int path = kernel_path(p, req_path);
+    if (path < 1) {
+        usdu::set_error("usdu_plan_split_worklists: this plan has no job-record kernels");
+        return USDU_ERR_UNSUPPORTED;
+    }
+    WorkList shorts, talls;
+    int s = crop_worklist(p, ids, n, B, path, LaunchModel{m.sm_count, path == 2 ? 16 : 0}, &shorts);
+    if (s == USDU_OK && path == 2) s = crop_worklist(p, ids, n, B, path, LaunchModel{m.sm_count, 32}, &talls);
+    if (s != USDU_OK) return s;
+    const WorkList& tall = path == 2 ? talls : shorts;
+    // short jobs by (output slot, column, first row): the short jobs inside a tall job's rows
+    std::map<std::array<int64_t, 3>, size_t> short_at;
+    int64_t all_outputs = 0;
+    for (size_t j = 0; j < (size_t)shorts.n_items(); ++j) {
+        const int32_t* r = shorts.items.data() + j * USDU_JOB_WORDS;
+        short_at[{(int64_t)(uint32_t)r[USDU_J_OFF_LO] | (int64_t)r[USDU_J_OFF_HI] << 32, r[USDU_J_OX_BASE], r[USDU_J_OY_BASE]}] = j;
+        all_outputs += job_outputs(r);
+    }
+    std::vector<std::pair<const WorkList*, size_t>> lj, ej;
+    if (n_prev == 0) {
+        for (size_t j = 0; j < (size_t)shorts.n_items(); ++j) lj.emplace_back(&shorts, j);
+    } else {
+        for (size_t j = 0; j < (size_t)tall.n_items(); ++j) {
+            const int32_t* r = tall.items.data() + j * USDU_JOB_WORDS;
+            if (!meets(p, r, prev, n_prev)) {
+                ej.emplace_back(&tall, j);
+                continue;
+            }
+            const int64_t slot = (int64_t)(uint32_t)r[USDU_J_OFF_LO] | (int64_t)r[USDU_J_OFF_HI] << 32;
+            int64_t covered = 0;
+            for (auto it = short_at.lower_bound({slot, r[USDU_J_OX_BASE], r[USDU_J_OY_BASE]});
+                 it != short_at.end() && it->first[0] == slot && it->first[1] == r[USDU_J_OX_BASE] &&
+                 it->first[2] < (int64_t)r[USDU_J_OY_BASE] + r[USDU_J_ROWS_OUT];
+                 ++it) {
+                const int32_t* q = shorts.items.data() + it->second * USDU_JOB_WORDS;
+                (meets(p, q, prev, n_prev) ? lj : ej).emplace_back(&shorts, it->second);
+                covered += job_outputs(q);
+            }
+            if (covered != job_outputs(r)) {
+                usdu::set_error("usdu_plan_split_worklists: the short jobs of a tall crop job cover %lld of its %lld outputs",
+                                (long long)covered, (long long)job_outputs(r));
+                return USDU_ERR_INVALID;
+            }
+        }
+    }
+    take_jobs(lj, shorts, all_outputs, late);
+    take_jobs(ej, tall, all_outputs, early);
+    int64_t outputs = 0;
+    for (const WorkList* wl : {late, early})
+        for (size_t j = 0; j < (size_t)wl->n_items(); ++j) outputs += job_outputs(wl->items.data() + j * USDU_JOB_WORDS);
+    if (outputs != all_outputs) {
+        usdu::set_error("usdu_plan_split_worklists: early and late jobs cover %lld of %lld outputs", (long long)outputs,
+                        (long long)all_outputs);
+        return USDU_ERR_INVALID;
+    }
+    if (path != 2) return blend_worklist(p, ids, offs, n, 4, B, path, 0, 0, m, blend);
+    // blend: cost(bh) = ceil(CTAs / resident slots) * (staged rows + written rows) per CTA
+    const int sms = m.sm_count > 0 ? m.sm_count : (usdu::sm_count() > 0 ? usdu::sm_count() : kDefaultSms);
+    const bool device = m.sm_count == 0 && usdu::sm_count() > 0;
+    int64_t best_cost = -1;
+    for (int bh : {32, 16}) {
+        WorkList wl;
+        if ((s = blend_worklist(p, ids, offs, n, 4, B, path, 0, 0, LaunchModel{m.sm_count, bh}, &wl)) != USDU_OK) return s;
+        if (wl.n_launch <= 0) {
+            *blend = std::move(wl);
+            return USDU_OK;
+        }
+        const int per_sm = usdu::mma::resident_ctas(USDU_KERNEL_BLEND, wl.ks2, (int)wl.patch_w, (int)wl.patch_h, bh, device);
+        if (per_sm < 0) return per_sm;
+        const int64_t slots = (int64_t)sms * std::max(per_sm, 1);
+        const int64_t cost = ceildiv(wl.n_launch * B, slots) * ((wl.patch_h & 0xFFFF) + bh);
+        if (best_cost < 0 || cost < best_cost) {
+            best_cost = cost;
+            *blend = std::move(wl);
+        }
+    }
+    return USDU_OK;
+}
+
 template <class F>
 int guarded(F&& f) {
     try {
@@ -1106,6 +1225,40 @@ int usdu_plan_blend_worklist(const usdu_plan* plan, const int32_t* tile_ids, con
             return r;
         }
         *wl = reinterpret_cast<usdu_worklist*>(w);
+        return (int)USDU_OK;
+    });
+}
+
+int usdu_plan_split_worklists(const usdu_plan* plan, const int32_t* tile_ids, const int64_t* src_offsets, int n,
+                              const int32_t* prev_ids, int n_prev, int B, int path, int sm_count, usdu_worklist** late,
+                              usdu_worklist** early, usdu_worklist** blend) {
+    const Plan* p = reinterpret_cast<const Plan*>(plan);
+    USDU_PLAN_ARG(p);
+    if (!late || !early || !blend) {
+        usdu::set_error("usdu_plan_split_worklists: an output handle is null");
+        return USDU_ERR_INVALID;
+    }
+    *late = *early = *blend = nullptr;
+    int s = check_ids(p, tile_ids, n, "usdu_plan_split_worklists");
+    if (s == USDU_OK) s = check_ids(p, prev_ids, n_prev, "usdu_plan_split_worklists (previous wave)");
+    if (s != USDU_OK) return s;
+    if ((n > 0 && !src_offsets) || B <= 0 || path < 1 || sm_count < 0) {
+        usdu::set_error("usdu_plan_split_worklists: bad arguments (B=%d path=%d sm_count=%d)", B, path, sm_count);
+        return USDU_ERR_INVALID;
+    }
+    return guarded([&]() {
+        WorkList *l = new WorkList(), *e = new WorkList(), *b = new WorkList();
+        const int r = split_worklists(const_cast<Plan*>(p), tile_ids, src_offsets, n, prev_ids, n_prev, B, path,
+                                      LaunchModel{sm_count, 0}, l, e, b);
+        if (r != USDU_OK) {
+            delete l;
+            delete e;
+            delete b;
+            return r;
+        }
+        *late = reinterpret_cast<usdu_worklist*>(l);
+        *early = reinterpret_cast<usdu_worklist*>(e);
+        *blend = reinterpret_cast<usdu_worklist*>(b);
         return (int)USDU_OK;
     });
 }

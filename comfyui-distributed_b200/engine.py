@@ -129,26 +129,21 @@ class DevicePlan:
         return self._wl[key]
 
     def split_lists(self, waves: Sequence[Sequence[int]], B: int, path_crop: int, path_blend: int):
-        """Per dependency wave, the work lists of the split schedule (planner.split_level), uploaded:
-        dict(crop=(wl, items), early / late = (wl, items) or None, offs, total, blend=(wl, items)),
-        or None when some wave does not run on job records."""
+        """Per dependency wave, the work lists of the split schedule (planner.split_lists), uploaded:
+        dict(crop=(wl, items) on the chain, early=(wl, items) beside the previous wave or None, offs, total,
+        blend=(wl, items)), or None when some list would not run on job records."""
         key = ("split", tuple(tuple(int(t) for t in w) for w in waves), B, path_crop, path_blend)
         if key not in self._wl:
-            out = []
-            for k, wave in enumerate(waves):
-                offs, _ = self.plan.slot_offsets(wave, B)
-                cr, coffs, ctotal, late, bl = self.plan.split_level(wave, offs, waves[k - 1] if k else None, B, path_crop)
-                if path_blend != path_crop:
-                    bl = self.plan.blend_worklist(wave, offs, 4, path_blend, B)
-                if cr.path < 1 or bl.path < 1:
-                    out = None
-                    break
-                e = {"crop": (cr, self._upload(cr)[0]), "offs": coffs, "total": ctotal, "early": None, "late": None,
-                     "blend": (bl, self._upload(bl)[0])}
-                if late is not None and late.any() and not late.all():
-                    we, wlate = self.plan.sub_worklist(cr, ~late), self.plan.sub_worklist(cr, late)
-                    e["early"], e["late"] = (we, self._upload(we)[0]), (wlate, self._upload(wlate)[0])
-                out.append(e)
+            out = None
+            if self.plan.kernel_path(path_crop) >= 1 and self.plan.kernel_path(path_blend) >= 1:
+                out = []
+                for k, wave in enumerate(waves):
+                    offs, _ = self.plan.slot_offsets(wave, B)
+                    chain, side, coffs, ctotal, bl = self.plan.split_lists(wave, offs, waves[k - 1] if k else None, B, path_crop)
+                    if path_blend != path_crop:
+                        bl = self.plan.blend_worklist(wave, offs, 4, path_blend, B)
+                    out.append({"crop": (chain, self._upload(chain)[0]), "offs": coffs, "total": ctotal,
+                                "early": None if side is None else (side, self._upload(side)[0]), "blend": (bl, self._upload(bl)[0])})
             self._wl[key] = out
         return self._wl[key]
 
@@ -422,7 +417,12 @@ class CastBands:
     (usdu_stream_args) that `set` rewrites before every replay, so one captured graph serves every caller's tensors."""
 
     def __init__(self, canvas: Canvas, order: Sequence[int], n_bands: int, max_ctas: int):
-        self.q, self.d = canvas.plan.stream_bands(order, canvas.B, n_bands, canvas.path_crop, canvas.path_blend)
+        # gated by the rows of the lists the graph launches: a taller early crop box reads rows the default lists do not
+        lists = canvas.dp.split_lists(split_waves(canvas.plan, order), canvas.B, canvas.path_crop, canvas.path_blend)
+        if lists is None:
+            raise nat.NativeError("canvas cast bands need the split schedule's job-record work lists")
+        levels = [([L["crop"][0]] + ([L["early"][0]] if L["early"] is not None else []), L["blend"][0]) for L in lists]
+        self.q, self.d = canvas.plan.stream_bands(order, canvas.B, n_bands, levels=levels)
         dev = canvas.buf.device
         self.args = torch.zeros(nat.STREAM_ARGS_BYTES, dtype=torch.uint8, device=dev)
         self.stream = torch.cuda.Stream(device=dev)
@@ -488,18 +488,25 @@ def use_split(canvas: Canvas, order: Sequence[int]) -> bool:
     return SCHEDULE == "split_crop" and canvas.path_crop >= 1 and canvas.path_blend >= 1 and len(canvas.plan.waves(order)) > 2
 
 
+def split_waves(plan: Plan, order: Sequence[int]) -> List[List[int]]:
+    """The dependency waves of `order` as run_split launches them: same-shape tiles adjacent."""
+    return [_sorted_by_shape(plan, w) for w in plan.waves(order)]
+
+
 def run_split(canvas: Canvas, order: Sequence[int], denoiser: Denoiser, s_early: "torch.cuda.Stream",
               casts: Optional[CastBands] = None) -> bool:
-    """run_progressive(order) with every level's crop launch split by dependency (planner.split_level); meant to be
+    """run_progressive(order) with every level's crop launch split by dependency (planner.split_lists); meant to be
     stream-captured.  single_gpu.py:40-64 orders a crop only after the blends that CHANGE pixels it reads:
     crop(k+1) = `late` jobs (their staged rectangle meets a feather support of wave k) + `early` jobs, which run on
     `s_early` beside sampler(k) / blend(k).  The chain per level shrinks to crop_late -> sampler -> blend (about a quarter
     of the crop jobs on cfg2).  A crop beside a blend only ever reads bytes whose value the blend leaves as it is.
+    The late jobs run in short blocks (latency: they are on the chain), the early ones in tall blocks (fewer staged rows:
+    they share the machine with blend(k)).
     False (nothing launched) when a wave has no job-record lists.
     casts: the canvas quantise / dequantise bands (CastBands) run inside the same graph: a crop waits for the quantise
     bands it reads, a dequantise band forks after the last blend that writes its rows."""
     plan, B = canvas.plan, canvas.B
-    waves = [_sorted_by_shape(plan, w) for w in plan.waves(order)]
+    waves = split_waves(plan, order)
     lists = canvas.dp.split_lists(waves, B, canvas.path_crop, canvas.path_blend)
     if lists is None:
         return False
@@ -515,11 +522,9 @@ def run_split(canvas: Canvas, order: Sequence[int], denoiser: Denoiser, s_early:
         buf = bufs[k]
         if casts is not None:
             casts.need(k, main)
+        canvas.crop_jobs(L["crop"][0], L["crop"][1], buf)
         if early_done[k] is not None:
-            canvas.crop_jobs(L["late"][0], L["late"][1], buf)
             main.wait_event(early_done[k])
-        else:
-            canvas.crop_jobs(L["crop"][0], L["crop"][1], buf)
         out = denoise_packed(plan, wave, buf, L["offs"], B, denoiser)
         if k + 1 < len(waves):                    # the crop jobs of wave k+1 that do not read what wave k changes
             N = lists[k + 1]

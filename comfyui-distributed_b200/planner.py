@@ -265,7 +265,8 @@ class Plan:
         return dataclasses.replace(wl, items=np.ascontiguousarray(J[mask]), algo_bytes=int(wl.algo_bytes * keep / max(J.shape[0], 1)))
 
     def split_level(self, wave: Sequence[int], offs: np.ndarray, prev: Optional[Sequence[int]], B: int, path: int = 2):
-        """Work lists of one dependency wave for the split schedule (engine.run_split).
+        """Work lists of one dependency wave split by dependency on ONE crop geometry (split_lists sizes the two parts
+        by role instead; this form is what tests/planner_model.py restates).
         -> (crop, offs, total, late mask or None, blend).
         crop jobs: `late` ones read pixels the previous wave `prev` changes, the rest may run beside the previous wave's
         sampler and blend."""
@@ -273,43 +274,66 @@ class Plan:
         late = self.crop_split(cr, prev) if (prev and cr.path >= 1) else None
         return cr, coffs, ctotal, late, self.blend_worklist(wave, offs, 4, path, B)
 
+    def split_lists(self, wave: Sequence[int], offs: np.ndarray, prev: Optional[Sequence[int]], B: int, path: int = 2):
+        """Work lists of one dependency wave as engine.run_split launches it (usdu_plan_split_worklists), each sized for
+        its role: -> (chain crop, side crop or None, element offsets of the tiles' crop outputs, total elements, blend).
+        The side crop holds the jobs that read no pixel the previous wave `prev` changes and runs beside prev's sampler
+        and blend; the chain crop, in short blocks, holds the rest (every job of the first wave, or of a wave whose jobs
+        all do).  Together they cover every crop output once.  path >= 1 (job records)."""
+        late, early, blend = self._native.split_worklists(wave, offs, prev or [], B, path, self._launch_model()[0])
+        late_wl, early_wl = self._worklist(late, False), self._worklist(early, False)
+        chain, side = late_wl, early_wl
+        if not len(late_wl.items):
+            chain, side = early_wl, None
+        elif not len(early_wl.items):
+            side = None
+        return chain, side, late["slots"], int(late["info"][nat.WL_TOTAL]), self._worklist(blend, True)
+
     CROP_BOX_ROWS = (0, 40, 48)           # rows of a crop's bulk-tensor box per kernel path (usdu_fast.cu / usdu_mma.cu kBoxR)
 
-    def wave_rows(self, waves: Sequence[Sequence[int]], B: int, path_crop: int = 2, path_blend: int = 2):
-        """Per dependency wave, the canvas rows its launches can touch (job records of the crop and blend work lists,
-        path >= 1): -> (touch, write), bool [len(waves), H].  touch = rows a crop's TMA box can load (the whole box from its
-        first staged row, plus the next row for the integer-pipe staging's 16-byte over-read) or a blend block loads;
-        write = rows of whole blend blocks, which a blend stores back even where the mask leaves them unchanged."""
-        touch = np.zeros((len(waves), self.H), dtype=bool)
-        write = np.zeros((len(waves), self.H), dtype=bool)
-        for k, wave in enumerate(waves):
-            cr, offs, _ = self.crop_worklist(wave, B, path_crop)
-            bl = self.blend_worklist(wave, offs, 4, path_blend, B)
-            if cr.path < 1 or bl.path < 1:
+    def wave_rows(self, levels: Sequence[Tuple[Sequence[WorkList], WorkList]]):
+        """Per dependency wave, the canvas rows its launches can touch.  levels[k] = (the crop work lists wave k launches,
+        its blend work list), job records (path >= 1) -> (touch, write), bool [len(levels), H].  touch = rows a crop's TMA
+        box can load (the whole box from its first staged row, plus the next row for the integer-pipe staging's 16-byte
+        over-read) or a blend block loads; write = rows of whole blend blocks, which a blend stores back even where the
+        mask leaves them unchanged."""
+        touch = np.zeros((len(levels), self.H), dtype=bool)
+        write = np.zeros((len(levels), self.H), dtype=bool)
+        for k, (crops, bl) in enumerate(levels):
+            if bl.path < 1 or any(cr.path < 1 for cr in crops):
                 raise ValueError("wave_rows needs job-record work lists (path >= 1)")
-            J = cr.items.reshape(-1, nat.JOB_WORDS)
-            box, slack = self.CROP_BOX_ROWS[cr.path], int(cr.path == 1)
-            for y0, n in zip(J[:, nat.J_SRC_B].tolist(), J[:, nat.J_ROWS].tolist()):
-                touch[k, max(y0, 0):min(y0 + max(n, box) + slack, self.H)] = True
+            for cr in crops:
+                J = cr.items.reshape(-1, nat.JOB_WORDS)
+                box, slack = self.CROP_BOX_ROWS[cr.path], int(cr.path == 1)
+                for y0, n in zip(J[:, nat.J_SRC_B].tolist(), J[:, nat.J_ROWS].tolist()):
+                    touch[k, max(y0, 0):min(y0 + max(n, box) + slack, self.H)] = True
             J = bl.items.reshape(-1, nat.JOB_WORDS)
             for y0, n in zip(J[:, nat.J_DST_Y].tolist(), J[:, nat.J_ROWS_OUT].tolist()):
                 write[k, max(y0, 0):min(y0 + max(n, bl.block_rows), self.H)] = True
             touch[k] |= write[k]
         return touch, write
 
-    def stream_bands(self, order: Optional[Sequence[int]], B: int, n_bands: int, path_crop: int = 2, path_blend: int = 2):
+    def stream_bands(self, order: Optional[Sequence[int]], B: int, n_bands: int, path_crop: int = 2, path_blend: int = 2,
+                     levels: Optional[Sequence[Tuple[Sequence[WorkList], WorkList]]] = None):
         """Row bands of the canvas quantise and dequantise passes when they run beside the level waves of `order`
         (engine.run_split).  -> (quantise, dequantise), lists of (y0, y1, wave): each quantise band [y0, y1) is tagged
         with the FIRST wave that touches one of its rows (it must be complete before that wave's crops start), each
         dequantise band with the LAST wave that writes one of its rows (it may start once that wave's blend is done).
         Rows are those of every frame; each list covers [0, H) once, top to bottom.  The first quantise band is exactly
         the rows the first wave touches (from row 0) and the last dequantise band the rows from the last wave's first
-        written row down; the rest of each pass is cut into n_bands - 1 bands of equal height."""
-        waves = self.waves(order)
-        touch, write = self.wave_rows(waves, B, path_crop, path_blend)
+        written row down; the rest of each pass is cut into n_bands - 1 bands of equal height.
+        levels: the work lists the waves launch (see wave_rows); None = one crop and one blend list per wave of `order`
+        as crop_worklist / blend_worklist build them."""
+        if levels is None:
+            levels = []
+            for wave in self.waves(order):
+                cr, offs, _ = self.crop_worklist(wave, B, path_crop)
+                levels.append(([cr], self.blend_worklist(wave, offs, 4, path_blend, B)))
+        touch, write = self.wave_rows(levels)
+        n_waves = len(levels)
         H, n_bands = self.H, max(1, int(n_bands))
-        lo = np.arange(len(waves))[:, None]
-        first = np.where(touch, lo, len(waves)).min(0)          # per row: first wave touching it
+        lo = np.arange(n_waves)[:, None]
+        first = np.where(touch, lo, n_waves).min(0)              # per row: first wave touching it
         last = np.where(write, lo, -1).max(0)                    # per row: last wave writing it
         if (last < 0).any():
             raise ValueError("stream_bands: some canvas row is written by no wave")
@@ -342,3 +366,4 @@ _PLAN_CACHE: LruCache[Plan] = LruCache(16)
 def get_plan(W: int, H: int, tile_width: int, tile_height: int, padding: int, mask_blur: int, uniform: bool) -> Plan:
     key = (W, H, tile_width, tile_height, padding, mask_blur, bool(uniform))
     return _PLAN_CACHE.get_or_build(key, lambda: Plan.build(*key))
+

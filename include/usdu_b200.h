@@ -35,7 +35,7 @@ extern "C" {
 #pragma GCC visibility push(default) /* the library itself is built with -fvisibility=hidden */
 #endif
 
-#define USDU_ABI_VERSION 14
+#define USDU_ABI_VERSION 15
 
 typedef enum usdu_status {
     USDU_OK = 0,
@@ -160,6 +160,17 @@ const char* usdu_last_error(void);
 int usdu_device_count(void);
 /* streaming multiprocessors of the current CUDA device, or a negative usdu_status */
 int usdu_sm_count(void);
+
+/* Resident CTAs per SM of a tensor-core kernel build at the dynamic shared memory its launcher requests for the patch
+ * words of a work list (USDU_WL_PATCH_W / _H; block_rows: the blend's block height): kernel = USDU_KERNEL_CROP_LDG,
+ * USDU_KERNEL_CROP_TMA (| USDU_KERNEL_LARGE: the 4-CTA build of launches of >= 8 CTAs per SM) or USDU_KERNEL_BLEND
+ * (fp32 sources); two_ksteps: the USDU_FLAG_MMA_KS2 build.  use_device = 1: the current device's occupancy calculator;
+ * 0: the table of the kernels' launch bounds and 228 KB of shared memory per SM.  0 = does not fit an SM. */
+#define USDU_KERNEL_CROP_LDG 0
+#define USDU_KERNEL_CROP_TMA 1
+#define USDU_KERNEL_BLEND 2
+#define USDU_KERNEL_LARGE 4
+int usdu_mma_resident_ctas(int kernel, int two_ksteps, int patch_w, int patch_h, int block_rows, int use_device);
 
 /* ---- host-side table builders (exact Pillow arithmetic, C double / C float) -------- */
 /* taps per output for an in->out LANCZOS axis (Resample.c: ceil(3*max(in/out,1))*2+1) */
@@ -460,6 +471,19 @@ int usdu_plan_blend_worklist(const usdu_plan* plan, const int32_t* tile_ids, con
                              int src_bytes, int B, int path, int part_i, int part_n, int sm_count,
                              int mma_block_rows, usdu_worklist** wl);
 int usdu_worklist_destroy(usdu_worklist* wl);
+/* Work lists of one dependency wave of the split schedule, which runs the crop jobs that read no pixel the previous
+ * wave's blend changes ("early") beside that wave's sampler and blend, and the rest ("late") on the chain
+ * crop -> sampler -> blend.  prev_ids[0..n_prev) = the previous wave (n_prev = 0: the first wave, every job is late);
+ * src_offsets as for the blend (fp32 sources).  The tensor-core path sizes each list for its role: late jobs in short
+ * blocks (16 rows), early jobs in the tallest the crop's 48-row box allows (usdu_plan_crop_worklist with 32 rows), a
+ * tall job that reads pixels of the previous wave's feather supports falls back to its short jobs, each late or early
+ * by its own rectangle; the blend block height minimises rounds of resident CTAs (usdu_mma_resident_ctas) times the
+ * rows a CTA stages and writes.  The integer-pipe path splits one list built as usdu_plan_crop_worklist does.  Early
+ * and late cover every crop output element exactly once and share the output layout (usdu_worklist_slots of either);
+ * `early` may have no items.  path >= 1 (job records). */
+int usdu_plan_split_worklists(const usdu_plan* plan, const int32_t* tile_ids, const int64_t* src_offsets, int n,
+                              const int32_t* prev_ids, int n_prev, int B, int path, int sm_count, usdu_worklist** late,
+                              usdu_worklist** early, usdu_worklist** blend);
 #define USDU_WL_INFO_WORDS 16      /* int64 words of usdu_worklist_info */
 #define USDU_WL_ITEMS 0            /* rows of usdu_worklist_items */
 #define USDU_WL_ITEM_WORDS 1       /* int32 per row: USDU_JOB_WORDS, USDU_CROP_ITEM_WORDS or USDU_BLEND_ITEM_WORDS */
