@@ -16,7 +16,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libusdu_b200.so")
 
 # constants mirrored from include/usdu_b200.h (checked against the header in tests)
-ABI_VERSION = 15
+ABI_VERSION = 16
 ERR_INVALID = -1
 CANVAS_SLACK = 16
 PLAN_INFO_WORDS = 16
@@ -94,6 +94,8 @@ _SIGNATURES = {
     "usdu_png_base64_u8": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "usdu_png_decode_u8": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "usdu_png_decode_warps": (c_int, [c_int]),
+    "usdu_png_encode_u8": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int64, c_void_p, c_int, c_void_p,
+                                   c_int, POINTER(c_int64), c_void_p, c_void_p, c_void_p]),
     "usdu_gather_unpack_f32": (c_int, [c_void_p, c_int, c_int64, c_void_p, c_void_p]),
     "usdu_t0_denoise": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_float, c_void_p]),
     "usdu_mask_scratch_bytes": (c_int64, [POINTER(c_int32), c_int]),
@@ -480,6 +482,19 @@ PNG_MAX_ROW_BYTES = 65536      # 16,384 px (ComfyUI's MAX_RESOLUTION) at 4 chann
 def png_decode_u8(src_ptr, segs_ptr, n_segs, descs_ptr, n, max_row_bytes, dst_ptr, stream):
     _check(lib().usdu_png_decode_u8(src_ptr, segs_ptr, n_segs, descs_ptr, n, max_row_bytes, dst_ptr, stream),
            "usdu_png_decode_u8")
+
+
+def png_encode_scratch_bytes(B: int, H: int, W: int) -> int:
+    """Device scratch usdu_png_encode_u8 takes for B RGB frames [H, W, 3]."""
+    raw = H * (1 + 3 * W)
+    return B * ((raw + 15) // 16 * 16 + 8 * H + 16)
+
+
+def png_encode_u8(src_ptr, B, H, W, C, template_ptr, png_len, runs_ptr, n_runs, chunks_ptr, n_chunks, adler_at,
+                  scratch_ptr, dst_ptr, stream):
+    at = (c_int64 * 4)(*[int(v) for v in adler_at])
+    _check(lib().usdu_png_encode_u8(src_ptr, B, H, W, C, template_ptr, png_len, runs_ptr, n_runs, chunks_ptr, n_chunks,
+                                    at, scratch_ptr, dst_ptr, stream), "usdu_png_encode_u8")
 
 
 def png_decode_warps(max_row_bytes: int) -> int:

@@ -1,4 +1,5 @@
-// usdu_png.cu -- u8 frames -> base64 text of a stored (deflate level 0, filter "None") PNG, on the device.
+// usdu_png.cu -- u8 frames -> PNG files on the device: base64 text of a stored (deflate level 0, filter "None") PNG for
+// the collector worker, and Pillow's level-0 PNG, filters and all, for the HTTP tile worker (the second half of the file).
 //
 // The reference's collector worker sends every image as base64 of a PIL PNG at compress_level=0
 // (nodes/collector.py:84-119).  At level 0 the deflate blocks are stored, so a PNG is layout plus two checksums:
@@ -20,6 +21,14 @@
 // message is ~raw of the message with its first 4 bytes inverted.  The chunk body (type + data) is right-aligned in a
 // zero-padded shared buffer of kPngThreads fixed-size segments; each thread CRCs one segment and the segments combine
 // with the compile-time multipliers x^(8 * kSeg * 2^j).
+//
+// Pillow's level-0 PNG (usdu_png_encode_u8) has a framing the host reads off Pillow for the shape (http_worker.png_layout),
+// so the kernels only fill it in:
+//   Pass 1  png_filter_kernel       one warp per row: Pillow's filter choice, the filtered row into R (scratch), the
+//                                   row's Adler partials.
+//   Pass 2  png_adler_frame_kernel  one CTA per frame: the Adler-32 of R, the template bytes outside the IDAT chunks.
+//   Pass 3  png_chunk_kernel        one CTA per (IDAT chunk, frame): template + R + Adler bytes spliced in shared
+//                                   memory, the chunk's CRC as above, the chunk written.
 #include "usdu_common.cuh"
 
 namespace usdu {
@@ -54,6 +63,74 @@ __device__ __forceinline__ uint32_t gf_mul(uint32_t a, uint32_t b) {
         b = (b >> 1) ^ ((b & 1u) ? kCrcPoly : 0u);
     }
     return p;
+}
+
+// x^(8 * kSpan): moves a raw CRC past one whole span (the filtered encoder's chunks may take several)
+constexpr uint32_t gf_mul_c(uint32_t a, uint32_t b) {
+    uint32_t p = 0;
+    for (int i = 0; i < 32; ++i) {
+        if (a & (0x80000000u >> i)) p ^= b;
+        b = (b >> 1) ^ ((b & 1u) ? kCrcPoly : 0u);
+    }
+    return p;
+}
+constexpr uint32_t kShift64 = gf_mul_c(kShift32, kShift32), kShift128 = gf_mul_c(kShift64, kShift64);
+constexpr uint32_t kShiftSpan = gf_mul_c(kShift128, kShift128);
+
+__device__ __forceinline__ void crc_table_init(uint32_t* table, int tid) {
+    for (int t = tid; t < 256; t += kPngThreads) {
+        uint32_t c = t;
+        for (int j = 0; j < 8; ++j) c = (c >> 1) ^ ((c & 1u) ? kCrcPoly : 0u);
+        table[t] = c;
+    }
+}
+
+// Raw CRC of the kSpan-byte shared buffer whose first s0 bytes are zero: each thread CRCs its kSeg-byte segment and the
+// segments combine in the warp; lane 0 returns its warp's raw CRC (span_crc_combine joins the warps).
+__device__ __forceinline__ uint32_t span_crc_warp(const uint32_t* body_words, const uint32_t* table, int tid,
+                                                  uint32_t s0) {
+    // segment i is followed by (kPngThreads - 1 - i) * kSeg bytes
+    uint32_t crc = 0;
+    if ((uint32_t)(tid + 1) * kSeg > s0) {
+        const uint32_t* seg = body_words + tid * (kSeg / 4);
+#pragma unroll 4
+        for (uint32_t i = 0; i < kSeg / 4; ++i) {
+            crc ^= seg[i];
+            crc = table[crc & 0xff] ^ (crc >> 8);
+            crc = table[crc & 0xff] ^ (crc >> 8);
+            crc = table[crc & 0xff] ^ (crc >> 8);
+            crc = table[crc & 0xff] ^ (crc >> 8);
+        }
+    }
+    crc = gf_mul(kShift1, crc) ^ __shfl_down_sync(0xffffffffu, crc, 1);
+    crc = gf_mul(kShift2, crc) ^ __shfl_down_sync(0xffffffffu, crc, 2);
+    crc = gf_mul(kShift4, crc) ^ __shfl_down_sync(0xffffffffu, crc, 4);
+    crc = gf_mul(kShift8, crc) ^ __shfl_down_sync(0xffffffffu, crc, 8);
+    crc = gf_mul(kShift16, crc) ^ __shfl_down_sync(0xffffffffu, crc, 16);
+    return crc;
+}
+
+__device__ __forceinline__ uint32_t span_crc_combine(const uint32_t* warp_crc) {
+    uint32_t c = 0;
+    for (int w = 0; w < kPngThreads / 32; ++w) c = gf_mul(kShift32, c) ^ warp_crc[w];
+    return c;
+}
+
+// m bytes of the shared buffer from byte src0 on to global g, with aligned word stores where g allows
+__device__ __forceinline__ void copy_out(uint8_t* g, const uint32_t* body_words, uint32_t src0, uint32_t m, int tid) {
+    const uint8_t* body = reinterpret_cast<const uint8_t*>(body_words);
+    uint32_t head = (4u - (uint32_t)((uintptr_t)g & 3)) & 3u;
+    head = head < m ? head : m;
+    const uint32_t nw = (m - head) / 4;
+    for (uint32_t i = tid; i < head; i += kPngThreads) g[i] = body[src0 + i];
+    {
+        const uint32_t so = src0 + head;
+        const uint32_t sh = (so & 3u) * 8u;
+        const uint32_t* sw = body_words + (so >> 2);
+        uint32_t* gw = reinterpret_cast<uint32_t*>(g + head);
+        for (uint32_t i = tid; i < nw; i += kPngThreads) gw[i] = __funnelshift_r(sw[i], sw[i + 1], sh);
+    }
+    for (uint32_t i = head + 4 * nw + tid; i < m; i += kPngThreads) g[i] = body[src0 + i];
 }
 
 __device__ __forceinline__ uint32_t crc_bitwise(uint32_t c, const uint8_t* p, int n) {
@@ -120,11 +197,7 @@ png_idat_kernel(const uint8_t* __restrict__ src, int64_t frame_bytes, uint32_t r
     const uint32_t n = 4 + hdr + L;                       // CRC'd bytes: chunk type + data
     const uint32_t s0 = kSpan - n;                        // the body is right-aligned; zeros before it
 
-    for (int t = tid; t < 256; t += kPngThreads) {
-        uint32_t c = t;
-        for (int j = 0; j < 8; ++j) c = (c >> 1) ^ ((c & 1u) ? kCrcPoly : 0u);
-        table[t] = c;
-    }
+    crc_table_init(table, tid);
     for (uint32_t w = tid; w < (s0 + 3) / 4; w += kPngThreads) body_words[w] = 0;
     if (tid == 0) body_words[kSpan / 4] = 0;              // slack word the funnel-shift copy may read
     __syncthreads();
@@ -161,24 +234,7 @@ png_idat_kernel(const uint8_t* __restrict__ src, int64_t frame_bytes, uint32_t r
     }
     __syncthreads();
 
-    // CRC of this thread's segment, then combine: segment i is followed by (kPngThreads - 1 - i) * kSeg bytes
-    uint32_t crc = 0;
-    if ((uint32_t)(tid + 1) * kSeg > s0) {
-        const uint32_t* seg = body_words + tid * (kSeg / 4);
-#pragma unroll 4
-        for (uint32_t i = 0; i < kSeg / 4; ++i) {
-            crc ^= seg[i];
-            crc = table[crc & 0xff] ^ (crc >> 8);
-            crc = table[crc & 0xff] ^ (crc >> 8);
-            crc = table[crc & 0xff] ^ (crc >> 8);
-            crc = table[crc & 0xff] ^ (crc >> 8);
-        }
-    }
-    crc = gf_mul(kShift1, crc) ^ __shfl_down_sync(0xffffffffu, crc, 1);
-    crc = gf_mul(kShift2, crc) ^ __shfl_down_sync(0xffffffffu, crc, 2);
-    crc = gf_mul(kShift4, crc) ^ __shfl_down_sync(0xffffffffu, crc, 4);
-    crc = gf_mul(kShift8, crc) ^ __shfl_down_sync(0xffffffffu, crc, 8);
-    crc = gf_mul(kShift16, crc) ^ __shfl_down_sync(0xffffffffu, crc, 16);
+    const uint32_t crc = span_crc_warp(body_words, table, tid, s0);
     s1 = warp_sum(s1);
     s2 = warp_sum(s2);
     if (lane == 0) {
@@ -191,25 +247,13 @@ png_idat_kernel(const uint8_t* __restrict__ src, int64_t frame_bytes, uint32_t r
     uint8_t* frame = staging + (int64_t)b * stride;
     uint8_t* g = frame + chunk_offset(k) + 8;
     const uint32_t m = n - 4, src0 = s0 + 4;
-    uint32_t head = (4u - (uint32_t)((uintptr_t)g & 3)) & 3u;
-    head = head < m ? head : m;
-    const uint32_t nw = (m - head) / 4;
-    for (uint32_t i = tid; i < head; i += kPngThreads) g[i] = body[src0 + i];
-    {
-        const uint32_t so = src0 + head;
-        const uint32_t sh = (so & 3u) * 8u;
-        const uint32_t* sw = body_words + (so >> 2);
-        uint32_t* gw = reinterpret_cast<uint32_t*>(g + head);
-        for (uint32_t i = tid; i < nw; i += kPngThreads) gw[i] = __funnelshift_r(sw[i], sw[i + 1], sh);
-    }
-    for (uint32_t i = head + 4 * nw + tid; i < m; i += kPngThreads) g[i] = body[src0 + i];
+    copy_out(g, body_words, src0, m, tid);
     __syncthreads();
 
     if (tid == 0) {
-        uint32_t c = 0;
+        const uint32_t c = span_crc_combine(warp_crc);
         unsigned long long t1 = 0, t2 = 0;
         for (int w = 0; w < kPngThreads / 32; ++w) {
-            c = gf_mul(kShift32, c) ^ warp_crc[w];
             t1 += warp_s1[w];
             t2 += warp_s2[w];
         }
@@ -320,6 +364,214 @@ png_base64_kernel(const uint8_t* __restrict__ staging, int64_t stride, int64_t p
     }
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Pillow's level-0 PNG of an RGB frame (usdu_png_encode_u8): the filtered stream R spliced into a framing the host
+// derived from Pillow for this shape.
+// ---------------------------------------------------------------------------------------------------------------------
+constexpr int kRowsPerCta = kPngThreads / 32;
+
+__device__ __forceinline__ uint32_t filter_cost(uint32_t v) {
+    v &= 0xffu;
+    return v < 128u ? v : 256u - v;
+}
+
+__device__ __forceinline__ uint32_t paeth_pred(uint32_t a, uint32_t b, uint32_t c) {
+    const int p = (int)a + (int)b - (int)c;
+    const int pa = abs(p - (int)a), pb = abs(p - (int)b), pc = abs(p - (int)c);
+    return (pa <= pb && pa <= pc) ? a : (pb <= pc ? b : c);
+}
+
+// Pass 1, one warp per row: the four filter sums in one sweep over the row and the raw row above, Pillow's choice, then
+// the filter byte and the filtered row to R[row * rowlen, ...) in the frame's scratch, and the row's Adler partials
+// (s1 = sum d, s2 = sum (rowlen - j) d_j, both mod 65521) to the frame's partial table.
+__global__ void __launch_bounds__(kPngThreads)
+png_filter_kernel(const uint8_t* __restrict__ src, int H, uint32_t row_bytes, uint8_t* __restrict__ scratch,
+                  int64_t stride, int64_t parts_at) {
+    const int lane = threadIdx.x & 31;
+    const int row = blockIdx.x * kRowsPerCta + (threadIdx.x >> 5);
+    if (row >= H) return;
+    const int b = blockIdx.y;
+    const uint8_t* cur = src + ((int64_t)b * H + row) * row_bytes;
+    const uint8_t* prev = cur - row_bytes;
+    const bool top = row == 0;
+    uint32_t s_none = 0, s_up = 0, s_sub = 0, s_paeth = 0;
+    for (uint32_t i = lane; i < row_bytes; i += 32) {
+        const uint32_t x = __ldg(cur + i);
+        const uint32_t a = i >= 3 ? __ldg(cur + i - 3) : 0u;
+        const uint32_t u = top ? 0u : __ldg(prev + i);
+        const uint32_t c = (top || i < 3) ? 0u : __ldg(prev + i - 3);
+        s_none += filter_cost(x);
+        s_up += filter_cost(x - u);
+        s_sub += filter_cost(x - a);
+        s_paeth += filter_cost(x - paeth_pred(a, u, c));
+    }
+    s_none = __reduce_add_sync(0xffffffffu, s_none);      // < 2^23 for rows of at most USDU_PNG_MAX_ROW_BYTES
+    s_up = __reduce_add_sync(0xffffffffu, s_up);
+    s_sub = __reduce_add_sync(0xffffffffu, s_sub);
+    s_paeth = __reduce_add_sync(0xffffffffu, s_paeth);
+    // Pillow tries None, Up, Sub, Paeth in this order and keeps a later one only when its sum is strictly smaller
+    uint32_t f = 0, best = s_none;
+    if (s_up < best) { f = 2; best = s_up; }
+    if (s_sub < best) { f = 1; best = s_sub; }
+    if (s_paeth < best) f = 4;
+
+    const uint32_t rowlen = row_bytes + 1;
+    uint8_t* frame = scratch + (int64_t)b * stride;
+    uint8_t* out = frame + (int64_t)row * rowlen;
+    uint32_t s1 = 0;
+    unsigned long long s2 = 0;
+    for (uint32_t i = lane; i < row_bytes; i += 32) {
+        const uint32_t x = __ldg(cur + i);
+        uint32_t v = x;
+        if (f == 2) {
+            v = x - (top ? 0u : __ldg(prev + i));
+        } else if (f == 1) {
+            v = x - (i >= 3 ? __ldg(cur + i - 3) : 0u);
+        } else if (f == 4) {
+            const uint32_t a = i >= 3 ? __ldg(cur + i - 3) : 0u;
+            const uint32_t u = top ? 0u : __ldg(prev + i);
+            const uint32_t c = (top || i < 3) ? 0u : __ldg(prev + i - 3);
+            v = x - paeth_pred(a, u, c);
+        }
+        v &= 0xffu;
+        out[1 + i] = (uint8_t)v;
+        s1 += v;
+        s2 += (unsigned long long)(rowlen - 1 - i) * v;
+    }
+    if (lane == 0) {
+        out[0] = (uint8_t)f;
+        s1 += f;
+        s2 += (unsigned long long)rowlen * f;
+    }
+    s1 = __reduce_add_sync(0xffffffffu, s1);               // < 2^25
+    s2 = warp_sum(s2);
+    if (lane == 0) {
+        uint32_t* part = reinterpret_cast<uint32_t*>(frame + parts_at) + 2 * row;
+        part[0] = s1 % kAdlerMod;
+        part[1] = (uint32_t)(s2 % kAdlerMod);
+    }
+}
+
+// Pass 2, one CTA per frame: the Adler-32 of R from the row partials (same fold as png_frame_kernel, with a_r = r *
+// rowlen and L_r = rowlen) into the frame's scratch word, and the template bytes outside every IDAT chunk (signature,
+// IHDR, whatever lies between or after the chunks) into the output.
+__global__ void __launch_bounds__(kPngThreads)
+png_adler_frame_kernel(int H, uint32_t rowlen, uint8_t* __restrict__ scratch, int64_t stride, int64_t parts_at,
+                       const uint8_t* __restrict__ tmpl, int64_t png_len, const int64_t* __restrict__ chunks,
+                       int n_chunks, uint8_t* __restrict__ dst) {
+    __shared__ unsigned long long red1[kPngThreads / 32], red2[kPngThreads / 32];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int b = blockIdx.x;
+    uint8_t* frame = scratch + (int64_t)b * stride;
+    const uint32_t* part = reinterpret_cast<const uint32_t*>(frame + parts_at);
+    const int64_t raw = (int64_t)H * rowlen;
+    unsigned long long A = 0, Bs = 0;
+    for (int r = tid; r < H; r += kPngThreads) {
+        const unsigned long long after = (unsigned long long)(raw - (int64_t)(r + 1) * rowlen) % kAdlerMod;
+        A = (A + part[2 * r]) % kAdlerMod;
+        Bs = (Bs + part[2 * r + 1] + after * part[2 * r]) % kAdlerMod;
+    }
+    A = warp_sum(A);
+    Bs = warp_sum(Bs);
+    if (lane == 0) {
+        red1[warp] = A;
+        red2[warp] = Bs;
+    }
+
+    uint8_t* out = dst + (int64_t)b * png_len;
+    const int64_t head = chunks[0] < png_len ? chunks[0] : png_len;
+    for (int64_t i = tid; i < head; i += kPngThreads) out[i] = tmpl[i];
+    for (int k = warp; k < n_chunks; k += kPngThreads / 32) {
+        const int64_t lo = chunks[2 * k] + 12 + chunks[2 * k + 1];
+        int64_t hi = k + 1 < n_chunks ? chunks[2 * k + 2] : png_len;
+        hi = hi < png_len ? hi : png_len;
+        for (int64_t i = (lo > 0 ? lo : 0) + lane; i < hi; i += 32) out[i] = tmpl[i];
+    }
+    __syncthreads();
+    if (tid != 0) return;
+    for (int w = 1; w < kPngThreads / 32; ++w) {
+        A += red1[w];
+        Bs += red2[w];
+    }
+    const uint32_t s1 = (uint32_t)((1 + A) % kAdlerMod);
+    const uint32_t s2 = (uint32_t)(((unsigned long long)raw % kAdlerMod + Bs) % kAdlerMod);
+    *reinterpret_cast<uint32_t*>(frame + parts_at + 8 * (int64_t)H) = (s2 << 16) | s1;
+}
+
+struct AdlerAt {
+    int64_t p[4];        // file offsets of the Adler-32 bytes, most significant first
+};
+
+// Pass 3, one CTA per (IDAT chunk, frame): the chunk's type and data assembled in shared memory -- template bytes, R
+// over the runs that fall in the chunk, the Adler bytes that do -- its CRC with the segment-combined scheme, the chunk
+// written out.  A chunk longer than one span is done in spans aligned to its end; only the first is zero-padded.
+__global__ void __launch_bounds__(kPngThreads)
+png_chunk_kernel(const uint8_t* __restrict__ scratch, int64_t stride, int64_t adler_slot, const uint8_t* __restrict__ tmpl,
+                 int64_t png_len, const int64_t* __restrict__ runs, int n_runs, const int64_t* __restrict__ chunks,
+                 AdlerAt adler_at, uint8_t* __restrict__ dst) {
+    extern __shared__ uint32_t body_words[];              // kSpan bytes + one word of slack
+    __shared__ uint32_t table[256];
+    __shared__ uint32_t warp_crc[kPngThreads / 32];
+    __shared__ int first_run;
+    uint8_t* body = reinterpret_cast<uint8_t*>(body_words);
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int k = blockIdx.x, b = blockIdx.y;
+    const uint8_t* R = scratch + (int64_t)b * stride;
+    const uint32_t adler = *reinterpret_cast<const uint32_t*>(R + adler_slot);
+    uint8_t* out = dst + (int64_t)b * png_len;
+    const int64_t off = chunks[2 * k], len = chunks[2 * k + 1];
+    const int64_t lo0 = off + 4, end = off + 8 + len;     // CRC'd bytes: chunk type + data
+    if (off < 0 || len < 0 || end + 4 > png_len) return;  // not a chunk of this file: leave the output alone
+    const int64_t nwin = (end - lo0 + kSpan - 1) / kSpan;
+
+    crc_table_init(table, tid);
+    uint32_t total = 0;                                   // raw CRC so far (thread 0)
+    for (int64_t w = 0; w < nwin; ++w) {
+        const int64_t hi = end - (nwin - 1 - w) * (int64_t)kSpan;
+        const int64_t lo = hi - kSpan > lo0 ? hi - kSpan : lo0;
+        const uint32_t s0 = kSpan - (uint32_t)(hi - lo);  // the bytes are right-aligned; zeros before them
+        for (uint32_t i = tid; i < (s0 + 3) / 4; i += kPngThreads) body_words[i] = 0;
+        if (tid == 0) {
+            body_words[kSpan / 4] = 0;                    // slack word the funnel-shift copy may read
+            int l = 0, h = n_runs;                        // first run ending after lo
+            while (l < h) {
+                const int m = (l + h) >> 1;
+                if (runs[3 * m] + runs[3 * m + 2] <= lo) l = m + 1; else h = m;
+            }
+            first_run = l;
+        }
+        __syncthreads();
+        for (int64_t p = lo + tid; p < hi; p += kPngThreads) body[s0 + (p - lo)] = tmpl[p];
+        __syncthreads();
+        for (int j = first_run; j < n_runs && runs[3 * j] < hi; ++j) {
+            const int64_t f = runs[3 * j], s = runs[3 * j + 1], n = runs[3 * j + 2];
+            const int64_t a = f > lo ? f : lo, e = f + n < hi ? f + n : hi;
+            for (int64_t p = a + tid; p < e; p += kPngThreads) body[s0 + (p - lo)] = R[s + (p - f)];
+        }
+        if (tid == 0) {
+            for (int i = 0; i < 4; ++i) {
+                const int64_t p = adler_at.p[i];
+                if (p >= lo && p < hi) body[s0 + (p - lo)] = (uint8_t)(adler >> (24 - 8 * i));
+            }
+            // the type bytes go in inverted: the CRC register's initial ~0 (see the top of the file); they are not
+            // copied out from here
+            for (int64_t p = lo0; p < lo0 + 4; ++p)
+                if (p >= lo && p < hi) body[s0 + (p - lo)] ^= 0xffu;
+        }
+        __syncthreads();
+        const uint32_t crc = span_crc_warp(body_words, table, tid, s0);
+        if (lane == 0) warp_crc[warp] = crc;
+        const int64_t d0 = lo > off + 8 ? lo : off + 8;   // chunk data in this span
+        if (hi > d0) copy_out(out + d0, body_words, s0 + (uint32_t)(d0 - lo), (uint32_t)(hi - d0), tid);
+        __syncthreads();
+        if (tid == 0) total = gf_mul(kShiftSpan, total) ^ span_crc_combine(warp_crc);
+    }
+    if (tid == 0) {
+        for (int i = 0; i < 8; ++i) out[off + i] = tmpl[off + i];   // length and type
+        put_be32(out + end, ~total);
+    }
+}
+
 }  // namespace
 }  // namespace usdu
 
@@ -366,6 +618,48 @@ int usdu_png_base64_u8(const uint8_t* src_dev, int B, int H, int W, int C, uint8
     const int grid = (int)(blocks < (int64_t)grid_sms() * 16 ? blocks : (int64_t)grid_sms() * 16);
     png_base64_kernel<<<grid, kPngThreads, 0, st>>>(staging_dev, g.stride, g.png_len, units, total, text_dev,
                                                     g.text_len);
+    USDU_CUDA(cudaGetLastError());
+    return USDU_OK;
+}
+
+int usdu_png_encode_u8(const uint8_t* src_dev, int B, int H, int W, int C, const uint8_t* template_dev, int64_t png_len,
+                       const int64_t* runs_dev, int n_runs, const int64_t* chunks_dev, int n_chunks,
+                       const int64_t* adler_at, uint8_t* scratch_dev, uint8_t* dst_dev, void* stream) {
+    USDU_REQUIRE(B >= 0 && B <= 65535, "usdu_png_encode_u8: batch %d outside [0, 65535]", B);
+    USDU_REQUIRE(C == 3, "usdu_png_encode_u8: %d channels: only RGB frames are encoded", C);
+    USDU_REQUIRE(H >= 1 && W >= 1, "usdu_png_encode_u8: empty frame %dx%d", W, H);
+    USDU_REQUIRE((int64_t)W * C <= USDU_PNG_MAX_ROW_BYTES, "usdu_png_encode_u8: rows of %lld bytes (at most %d)",
+                 (long long)W * C, USDU_PNG_MAX_ROW_BYTES);
+    const int64_t rowlen = (int64_t)W * C + 1, raw = (int64_t)H * rowlen;
+    USDU_REQUIRE(png_len > raw && n_runs >= 1 && n_chunks >= 1,
+                 "usdu_png_encode_u8: layout of %lld bytes, %d runs, %d chunks for a stream of %lld bytes",
+                 (long long)png_len, n_runs, n_chunks, (long long)raw);
+    USDU_REQUIRE(adler_at, "usdu_png_encode_u8: null pointer");
+    AdlerAt at;
+    for (int i = 0; i < 4; ++i) {
+        USDU_REQUIRE(adler_at[i] >= 0 && adler_at[i] < png_len, "usdu_png_encode_u8: Adler byte %d at %lld", i,
+                     (long long)adler_at[i]);
+        at.p[i] = adler_at[i];
+    }
+    if (B == 0) return USDU_OK;
+    USDU_REQUIRE(src_dev && template_dev && runs_dev && chunks_dev && scratch_dev && dst_dev,
+                 "usdu_png_encode_u8: null pointer");
+    USDU_REQUIRE(((uintptr_t)scratch_dev & 15) == 0, "usdu_png_encode_u8: scratch must be 16-byte aligned");
+    const int64_t parts_at = (raw + 15) / 16 * 16;
+    const int64_t stride = parts_at + 8 * (int64_t)H + 16;
+    cudaStream_t st = (cudaStream_t)stream;
+    png_filter_kernel<<<dim3((unsigned)((H + kRowsPerCta - 1) / kRowsPerCta), (unsigned)B), kPngThreads, 0, st>>>(
+        src_dev, H, (uint32_t)(W * C), scratch_dev, stride, parts_at);
+    USDU_CUDA(cudaGetLastError());
+    png_adler_frame_kernel<<<B, kPngThreads, 0, st>>>(H, (uint32_t)rowlen, scratch_dev, stride, parts_at, template_dev,
+                                                      png_len, chunks_dev, n_chunks, dst_dev);
+    USDU_CUDA(cudaGetLastError());
+    const size_t smem = kSpan + 4;
+    int r = raise_smem_limit((const void*)png_chunk_kernel, smem);
+    if (r != USDU_OK) return r;
+    png_chunk_kernel<<<dim3((unsigned)n_chunks, (unsigned)B), kPngThreads, smem, st>>>(
+        scratch_dev, stride, parts_at + 8 * (int64_t)H, template_dev, png_len, runs_dev, n_runs, chunks_dev, at,
+        dst_dev);
     USDU_CUDA(cudaGetLastError());
     return USDU_OK;
 }

@@ -731,7 +731,8 @@ class WorkerJob:
         B, H, W, _ = x.shape
         self.plan = get_plan(W, H, tile_width, tile_height, padding, mask_blur, force_uniform_tiles)
         self.denoiser = denoiser
-        self.times = {"device_ms": 0.0, "d2h_ms": 0.0, "tiles": 0}    # CUDA-event totals over step()
+        # CUDA-event totals over step() and step_png()
+        self.times = {"device_ms": 0.0, "encode_ms": 0.0, "d2h_ms": 0.0, "tiles": 0}
         with torch.cuda.device(self.device):
             if not x.is_cuda:                    # uploaded once; the canvas is all the job keeps
                 x = (x if x.is_pinned() else x.pin_memory()).to(self.device, non_blocking=True)
@@ -756,6 +757,37 @@ class WorkerJob:
         self.times["d2h_ms"] += e1.elapsed_time(e2)
         self.times["tiles"] += 1
         return host.numpy()
+
+    def step_png(self, tile_id: int):
+        """Process tile `tile_id` -> its B frames as the PNG files encode_png writes, encoded on the device
+        (http_worker.encode_png_gpu) on the same stream and brought back in one copy through page-locked memory.  For a
+        tile shape whose layout check failed (http_worker.png_layout) -> step(tile_id)'s u8 tiles, for PIL."""
+        from .http_worker import encode_png_gpu, png_layout
+        tile_id = int(tile_id)
+        if not 0 <= tile_id < len(self.plan.tiles):
+            raise ValueError(f"tile id {tile_id} is outside this job's {len(self.plan.tiles)} tiles")
+        t = self.plan.tiles[tile_id]
+        layout = png_layout(t.ph, t.pw, self.device)
+        if layout is None:
+            return self.step(tile_id)
+        B, n = self.canvas.B, layout.png_len
+        with torch.cuda.device(self.device):
+            e0, e1, e2, e3 = (torch.cuda.Event(enable_timing=True) for _ in range(4))
+            e0.record()
+            q = run_progressive(self.canvas, [tile_id], self.denoiser, keep_processed=True)[tile_id]
+            e1.record()
+            files = encode_png_gpu(q, layout, torch.empty(B * n, dtype=torch.uint8, device=self.device))
+            e2.record()
+            host = torch.empty(B * n, dtype=torch.uint8, pin_memory=True)
+            host.copy_(files, non_blocking=True)
+            e3.record()
+            e3.synchronize()
+        self.times["device_ms"] += e0.elapsed_time(e1)
+        self.times["encode_ms"] += e1.elapsed_time(e2)
+        self.times["d2h_ms"] += e2.elapsed_time(e3)
+        self.times["tiles"] += 1
+        data = host.numpy().tobytes()
+        return [data[b * n:(b + 1) * n] for b in range(B)]
 
     def step_device(self, tile_id: int):
         """Process tile `tile_id` into this canvas only (the master of HTTP workers: its tiles never leave the device).

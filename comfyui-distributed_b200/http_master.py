@@ -57,11 +57,14 @@ def heartbeat_interval() -> float:
 class PngInfo:
     """A validated 8-bit, non-interlaced PNG.  The filtered stream R (per row a filter byte, then W*C bytes) is the
     concatenation, in order, of data[src:src + length] for (src, raw start) in `segs` (each runs to the next raw start,
-    the last to |R|), or, when the stream had compressed blocks, `inflated` itself (segs = [(0, 0)])."""
-    __slots__ = ("W", "H", "C", "segs", "inflated")
+    the last to |R|), or, when the stream had compressed blocks, `inflated` itself (segs = [(0, 0)]).  `idat` lists the
+    (file offset, data length) of every IDAT chunk, `trailer` the file offsets of the four Adler-32 bytes (stored blocks
+    only, else None): the framing http_worker.png_layout reads."""
+    __slots__ = ("W", "H", "C", "segs", "inflated", "idat", "trailer")
 
-    def __init__(self, W, H, C, segs, inflated=None):
+    def __init__(self, W, H, C, segs, inflated=None, idat=(), trailer=None):
         self.W, self.H, self.C, self.segs, self.inflated = W, H, C, segs, inflated
+        self.idat, self.trailer = list(idat), trailer
 
     @property
     def raw_len(self) -> int:
@@ -122,8 +125,8 @@ def parse_png(data: bytes) -> PngInfo:
     W, H, C = ihdr
     raw_len = H * (1 + W * C)
     stream = _IdatStream(data, idat)
-    segs, inflated = _stored_segments(stream, raw_len)
-    info = PngInfo(W, H, C, segs, inflated)
+    segs, inflated, trailer = _stored_segments(stream, raw_len)
+    info = PngInfo(W, H, C, segs, inflated, [(off - 8, ln) for off, ln in idat], trailer)
     _check_filters(info, data)
     return info
 
@@ -164,7 +167,8 @@ class _IdatStream:
 
 
 def _stored_segments(st: _IdatStream, raw_len: int):
-    """-> (segments, None) for a zlib stream of stored blocks, or ([(0, 0)], R) after inflating any other stream."""
+    """-> (segments, None, file offsets of the Adler-32 bytes) for a zlib stream of stored blocks, or ([(0, 0)], R, None)
+    after inflating any other stream."""
     hdr = st.read(0, 2)
     cmf, flg = hdr[0], hdr[1]
     if (cmf & 0x0F) != 8 or (cmf >> 4) > 7 or (cmf * 256 + flg) % 31 != 0 or (flg & 0x20):
@@ -193,7 +197,8 @@ def _stored_segments(st: _IdatStream, raw_len: int):
         raise ValueError("image data is truncated")
     if struct.unpack(">I", st.read(pos, 4))[0] != adler:
         raise ValueError("bad Adler-32 of the image data")
-    return segs, None
+    trailer = [off + i for off, k in st.ranges(pos, 4) for i in range(k)]
+    return segs, None, trailer
 
 
 def _inflated(st: _IdatStream, raw_len: int):
@@ -206,7 +211,7 @@ def _inflated(st: _IdatStream, raw_len: int):
         raise ValueError("image data is truncated")
     if len(out) < raw_len:
         raise ValueError("image data is truncated")
-    return [(0, 0)], out[:raw_len]
+    return [(0, 0)], out[:raw_len], None
 
 
 def filtered_stream(info: PngInfo, data: bytes) -> bytes:

@@ -7,6 +7,10 @@ Blocking HTTP on the caller's thread (ComfyUI's prompt executor) with the standa
 the wire is what the reference's worker sends: the job-ready poll, one `request_image` per tile, a heartbeat after every
 tile, the processed tiles as level-0 PNGs in size-aware multipart chunks every COMFYUI_MAX_BATCH tiles, and `is_last` on
 the final chunk (or the empty completion signal).  Retry counts, delays and timeouts are the reference's.
+
+The tile PNGs are the bytes Pillow writes at compress_level=0.  They are encoded on the GPU (csrc/usdu_png.cu,
+usdu_png_encode_u8) into a framing read off the installed Pillow for each tile shape (`png_layout`); a shape whose framing
+fails its checks is PIL-encoded on the host, as before.
 """
 from __future__ import annotations
 
@@ -19,9 +23,12 @@ import urllib.error
 import urllib.parse
 import urllib.request
 import uuid
-from typing import Callable, Iterable, List, Optional, Sequence, Tuple
+import warnings
+from typing import Callable, Iterable, List, Optional, Sequence, Tuple, Union
 
 import numpy as np
+
+from .lru import LruCache
 
 JOB_POLL_INTERVAL = 1.0            # utils/constants.py:53-54
 JOB_POLL_MAX_ATTEMPTS = 20
@@ -34,8 +41,8 @@ CHUNK_HEADROOM = 1024 * 1024       # worker_comms.py:49
 TILE_OVERHEAD = 1024               # worker_comms.py:65
 COLLECTOR_TIMEOUT = 60.0           # one job_complete POST (collector.py:110-116)
 
-TileStep = Callable[[int], np.ndarray]
-"""step(tile id) -> the processed tile of every frame, uint8 [B, ph, pw, 3] on the host."""
+TileStep = Callable[[int], Union[np.ndarray, List[bytes]]]
+"""step(tile id) -> the processed tile of every frame, uint8 [B, ph, pw, 3] on the host, or already as B PNG files."""
 
 
 class HttpError(RuntimeError):
@@ -66,6 +73,179 @@ def encode_png(tile: np.ndarray) -> bytes:
     bio = io.BytesIO()
     Image.fromarray(np.ascontiguousarray(tile)).save(bio, format="PNG", compress_level=0)
     return bio.getvalue()
+
+
+# --------------------------------------------------------------------------------------
+# encode_png's bytes on the GPU: Pillow's framing for the shape + the filtered stream and checksums from the kernels
+# --------------------------------------------------------------------------------------
+class PngLayout:
+    """The framing of Pillow's level-0 PNG of an RGB frame [H, W, 3], in the tables usdu_png_encode_u8 takes (see
+    include/usdu_b200.h): `template` (a file of this shape), `runs` int64 [n, 3] (file offset, stream offset, length)
+    of the filtered stream R inside it, `chunks` int64 [n, 2] (file offset, data length) of every IDAT chunk, and
+    `adler_at`, the file offsets of the four Adler-32 bytes."""
+
+    def __init__(self, H: int, W: int, template: bytes, runs: np.ndarray, chunks: np.ndarray, adler_at: Sequence[int]):
+        self.H, self.W, self.template = int(H), int(W), bytes(template)
+        self.runs = np.ascontiguousarray(runs, np.int64).reshape(-1, 3)
+        self.chunks = np.ascontiguousarray(chunks, np.int64).reshape(-1, 2)
+        self.adler_at = [int(p) for p in adler_at]
+        self._device = {}
+        self._check()
+
+    @property
+    def png_len(self) -> int:
+        return len(self.template)
+
+    @property
+    def raw_len(self) -> int:
+        return self.H * (1 + 3 * self.W)
+
+    def _check(self):
+        """ValueError unless the tables are what the kernels assume: runs cover R once, in order, inside IDAT data;
+        the Adler bytes lie in IDAT data outside every run; chunks are sorted, disjoint and inside the file."""
+        n = self.png_len
+        if len(self.runs) == 0 or len(self.chunks) == 0 or len(self.adler_at) != 4:
+            raise ValueError("empty layout")
+        ends = self.runs[:, 1] + self.runs[:, 2]
+        if (self.runs[0, 1] != 0 or ends[-1] != self.raw_len or (self.runs[1:, 1] != ends[:-1]).any()
+                or (self.runs[:, 2] <= 0).any() or (np.diff(self.runs[:, 0]) <= 0).any()):
+            raise ValueError("the runs do not cover the filtered stream in order")
+        c_end = self.chunks[:, 0] + 12 + self.chunks[:, 1]
+        if (self.chunks[:, 0] < 0).any() or (self.chunks[:, 1] < 0).any() or c_end[-1] > n or \
+                (self.chunks[1:, 0] < c_end[:-1]).any():
+            raise ValueError("IDAT chunks overlap or leave the file")
+        data = np.zeros(n + 1, np.int64)              # +1 inside IDAT data, -1 (twice) for a run or Adler byte
+        for off, ln in self.chunks.tolist():
+            data[off + 8] += 1
+            data[off + 8 + ln] -= 1
+        in_data = np.cumsum(data)[:n] > 0
+        used = np.zeros(n + 1, np.int64)
+        for f, _, ln in self.runs.tolist():
+            used[f] += 1
+            used[f + ln] -= 1
+        used = np.cumsum(used)[:n]
+        used[self.adler_at] += 1
+        if (used > 1).any() or not in_data[used > 0].all():
+            raise ValueError("a run or an Adler byte lies outside IDAT data or on another one")
+
+    def framing(self) -> tuple:
+        """Everything that does not depend on pixel values: the tables and the template with R, the Adler bytes and
+        the IDAT CRCs blanked."""
+        t = np.frombuffer(self.template, np.uint8).copy()
+        for f, _, ln in self.runs.tolist():
+            t[f: f + ln] = 0
+        t[self.adler_at] = 0
+        for off, ln in self.chunks.tolist():
+            t[off + 8 + ln: off + 12 + ln] = 0
+        return (self.H, self.W, t.tobytes(), self.runs.tobytes(), self.chunks.tobytes(), tuple(self.adler_at))
+
+    def device_tables(self, device):
+        """(template, runs, chunks) on `device`, uploaded once per device."""
+        import torch
+        key = str(device)
+        if key not in self._device:
+            self._device[key] = tuple(torch.from_numpy(np.frombuffer(a, np.uint8).copy() if isinstance(a, bytes) else a)
+                                      .to(device) for a in (self.template, self.runs, self.chunks))
+        return self._device[key]
+
+
+def layout_from_png(data: bytes) -> PngLayout:
+    """The layout of one of Pillow's level-0 RGB PNGs, from http_master.parse_png's segment and chunk tables."""
+    from .http_master import parse_png
+    info = parse_png(data)
+    if info.C != 3 or info.inflated is not None:
+        raise ValueError("not a stored-block RGB PNG")
+    starts = [r for _, r in info.segs] + [info.raw_len]
+    runs = [(off, r, starts[i + 1] - r) for i, (off, r) in enumerate(info.segs)]
+    return PngLayout(info.H, info.W, data, np.asarray(runs, np.int64), np.asarray(info.idat, np.int64), info.trailer)
+
+
+def png_probe(H: int, W: int, variant: int = 0) -> np.ndarray:
+    """A u8 RGB frame [H, W, 3] on which, given seven rows and four columns or more, each of Pillow's filters None, Up,
+    Sub and Paeth wins on some row.  Rows cycle through noise, a duplicate of the row above (Up), a horizontal ramp
+    (Sub), a zero row, a row constant on its left half and noisy on its right, a row constant on its left half with
+    another value and a copy of the row above on its right (Paeth: Sub wins on the left, Up on the right), and values
+    126..130 (the cost's wrap).  Row 0, with zeros above it, ties None with Up and Sub with Paeth.  `variant` changes
+    the values, not the shape."""
+    v = int(variant) % 64
+    rng = np.random.default_rng(1000 + v)
+    x = np.arange(W, dtype=np.int64)[:, None]
+    half = W // 2
+    img = np.zeros((H, W, 3), np.uint8)
+    for r in range(H):
+        k = r % 7
+        if k == 0:
+            img[r] = rng.integers(0, 256, (W, 3))
+        elif k == 1:
+            img[r] = img[r - 1]
+        elif k == 2:
+            img[r] = (2 * x + 40 * v + np.array([0, 85, 170])) % 256
+        elif k == 4:
+            img[r, :half] = 50 + v
+            img[r, half:] = rng.integers(0, 256, (W - half, 3))
+        elif k == 5:
+            img[r, :half] = 180 + v
+            img[r, half:] = img[r - 1, half:]
+        elif k == 6:
+            img[r] = rng.integers(126, 131, (W, 3))
+    return img
+
+
+def encode_png_gpu(frames, layout: PngLayout, out, scratch=None):
+    """Enqueue usdu_png_encode_u8 on the current stream: frames = contiguous CUDA u8 [B, H, W, 3], out = CUDA u8 of at
+    least B * layout.png_len bytes, frame b's file at out[b * png_len:]."""
+    import torch
+    from . import _native as nat
+    B, H, W, C = frames.shape
+    if (H, W, C) != (layout.H, layout.W, 3) or frames.dtype != torch.uint8 or not frames.is_contiguous():
+        raise ValueError(f"frames {frames.dtype} {tuple(frames.shape)} do not fit a layout of {layout.H}x{layout.W}")
+    if out.numel() < B * layout.png_len:
+        raise ValueError(f"output of {out.numel()} bytes for {B} files of {layout.png_len}")
+    if scratch is None:
+        scratch = torch.empty(nat.png_encode_scratch_bytes(B, H, W), dtype=torch.uint8, device=frames.device)
+    tmpl, runs, chunks = layout.device_tables(frames.device)
+    nat.png_encode_u8(frames.data_ptr(), B, H, W, 3, tmpl.data_ptr(), layout.png_len, runs.data_ptr(), len(layout.runs),
+                      chunks.data_ptr(), len(layout.chunks), layout.adler_at, scratch.data_ptr(), out.data_ptr(),
+                      torch.cuda.current_stream(frames.device).cuda_stream)
+    return out
+
+
+def _checked_layout(H: int, W: int, device) -> PngLayout:
+    """Pillow's framing for [H, W, 3], checked: two probes of different content must frame alike, and the kernels must
+    reproduce Pillow's bytes of both.  ValueError otherwise."""
+    import torch
+    probes = [png_probe(H, W, v) for v in (0, 1)]
+    files = [encode_png(p) for p in probes]
+    layout = layout_from_png(files[0])
+    if layout_from_png(files[1]).framing() != layout.framing():
+        raise ValueError("Pillow's framing depends on the pixel values")
+    with torch.cuda.device(device):
+        frames = torch.from_numpy(np.stack(probes)).to(device)
+        out = torch.empty(2 * layout.png_len, dtype=torch.uint8, device=device)
+        encode_png_gpu(frames, layout, out)
+        got = out.cpu().numpy().tobytes()
+    if got != b"".join(files):
+        raise ValueError("the GPU encoder's bytes differ from Pillow's")
+    return layout
+
+
+_LAYOUTS: LruCache = LruCache(32)
+
+
+def png_layout(H: int, W: int, device=None) -> Optional[PngLayout]:
+    """The checked layout of [H, W, 3] tiles, or None (after one warning per shape) when the installed Pillow's bytes
+    cannot be reproduced: that shape's tiles are then PIL-encoded on the host."""
+    import torch
+    device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+    key = (int(H), int(W), str(device))
+    if key in _LAYOUTS:
+        return _LAYOUTS.get(key)
+    try:
+        layout = _checked_layout(int(H), int(W), device)
+    except (ValueError, TypeError) as e:
+        warnings.warn(f"PNG tiles of {W}x{H} are encoded with PIL on the host: {e}", RuntimeWarning, stacklevel=2)
+        layout = None
+    return _LAYOUTS.put(key, layout)
 
 
 def multipart(parts: Sequence[Tuple[str, bytes, Optional[str], Optional[str]]]) -> Tuple[bytes, str]:
@@ -208,8 +388,8 @@ class HttpStaticWorker:
             i = j
 
     def run(self, step: TileStep) -> bool:
-        """Pull tile ids until the master's queue is empty, processing each with `step` and uploading the results.
-        False (nothing processed or sent) when the job never became ready, as static.py:222-224."""
+        """Pull tile ids until the master's queue is empty, processing each with `step` and uploading the results.  A
+        step returns either the u8 tiles (PIL-encoded here) or their B PNG files (WorkerJob.step_png).  False (nothing processed or sent) when the job never became ready, as static.py:222-224."""
         poll = _interrupt_poll()
         if not self.wait_ready():
             return False
@@ -230,13 +410,18 @@ class HttpStaticWorker:
             self.pulled.append(tile_id)
             out = step(tile_id)
             t2 = clock()
-            if out.dtype != np.uint8 or out.ndim != 4 or out.shape[0] != self.batch_size or out.shape[3] != 3:
-                raise ValueError(f"tile step returned {out.dtype} {tuple(out.shape)}, expected uint8 [{self.batch_size}, h, w, 3]")
+            if isinstance(out, (list, tuple)):
+                if len(out) != self.batch_size or not all(isinstance(f, (bytes, bytearray)) for f in out):
+                    raise ValueError(f"tile step returned {len(out)} items, expected {self.batch_size} PNG files")
+                pngs = [bytes(f) for f in out]
+            else:
+                if out.dtype != np.uint8 or out.ndim != 4 or out.shape[0] != self.batch_size or out.shape[3] != 3:
+                    raise ValueError(f"tile step returned {out.dtype} {tuple(out.shape)}, expected uint8 [{self.batch_size}, h, w, 3]")
+                pngs = [encode_png(out[b]) for b in range(self.batch_size)]
             x, y, ew, eh = self.geometry[tile_id]
             for b in range(self.batch_size):
-                pending.append((encode_png(out[b]), {"tile_idx": tile_id, "x": x, "y": y, "extracted_width": ew,
-                                                     "extracted_height": eh, "batch_idx": b,
-                                                     "global_idx": b * n_tiles + tile_id}))
+                pending.append((pngs[b], {"tile_idx": tile_id, "x": x, "y": y, "extracted_width": ew,
+                                          "extracted_height": eh, "batch_idx": b, "global_idx": b * n_tiles + tile_id}))
             t3 = clock()
             self.heartbeat()
             t4 = clock()

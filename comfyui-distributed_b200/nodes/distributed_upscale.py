@@ -130,7 +130,7 @@ class UltimateSDUpscaleDistributed:
                             device=dev)
             worker = HttpStaticWorker(master_url, multi_job_id, worker_id, padding,
                                       [(t.x1, t.y1, t.ew, t.eh) for t in job.plan.tiles], job.canvas.B)
-            worker.run(job.step)
+            worker.run(job.step_png)
             self.last_stats.update(pulled=list(worker.pulled), chunks=worker.chunks)
             return (upscaled_image,)
         if multi_job_id and not is_worker and world == 1 and json.loads(enabled_worker_ids) and http_master.serving():

@@ -35,7 +35,7 @@ extern "C" {
 #pragma GCC visibility push(default) /* the library itself is built with -fvisibility=hidden */
 #endif
 
-#define USDU_ABI_VERSION 15
+#define USDU_ABI_VERSION 16
 
 typedef enum usdu_status {
     USDU_OK = 0,
@@ -329,6 +329,28 @@ int usdu_png_base64_u8(const uint8_t* src_dev, int B, int H, int W, int C, uint8
 int usdu_png_decode_u8(const uint8_t* src_dev, const int64_t* segs_dev, int64_t n_segs, const int64_t* descs_dev,
                        int n, int max_row_bytes, uint8_t* dst_dev, void* stream);
 int usdu_png_decode_warps(int max_row_bytes);
+
+/* HTTP tile worker transport (upscale/worker_comms.py:30-34): each u8 RGB frame [H, W, 3] as the PNG Pillow writes with
+ * compress_level=0, byte for byte.  At level 0 Pillow's file is a framing that depends on the shape alone, filled with
+ * the filtered stream R and the checksums.  R is per row one filter byte and the row filtered with it (|R| = H*(1 + 3W));
+ * the kernels choose each row's filter as Pillow does without `optimize`: for None (0), Up (2), Sub (1), Paeth (4) in
+ * that order, the sum over the filtered bytes v of min(v, 256 - v), with the previous RAW row above (zeros above the
+ * first); the first candidate with the smallest sum.  This library does not model zlib or Pillow's buffering: the
+ * caller derives the framing from Pillow for the shape (one encoded probe) and passes it as a layout:
+ *   template_dev: png_len bytes, a file of this shape (its stream bytes and checksums are overwritten);
+ *   runs_dev: n_runs (file offset, stream offset, length) int64 triples, sorted by file offset: R[stream offset, + length)
+ *     goes to file[file offset, + length);
+ *   chunks_dev: n_chunks (file offset, data length) int64 pairs, sorted: every IDAT chunk, whose CRC-32 (over type and
+ *     data) is recomputed; every file byte outside the chunks is copied from the template;
+ *   adler_at (host): the 4 file offsets of the big-endian Adler-32 of R, most significant byte first.
+ * The runs, the Adler bytes and the stored-block headers may fall anywhere in the chunks, split across two of them
+ * included; runs and Adler bytes lie in chunk data and do not overlap.  src_dev = B contiguous u8 frames [H, W, 3];
+ * scratch_dev (16-byte aligned) = B * (round_up(|R|, 16) + 8*H + 16) bytes; frame b's file goes to dst_dev + b *
+ * png_len.  Three launches on `stream`, no host synchronisation.  USDU_ERR_INVALID unless C = 3, W*3 <=
+ * USDU_PNG_MAX_ROW_BYTES, 0 <= B <= 65535, png_len > |R| and the Adler offsets lie in the file. */
+int usdu_png_encode_u8(const uint8_t* src_dev, int B, int H, int W, int C, const uint8_t* template_dev, int64_t png_len,
+                       const int64_t* runs_dev, int n_runs, const int64_t* chunks_dev, int n_chunks,
+                       const int64_t* adler_at, uint8_t* scratch_dev, uint8_t* dst_dev, void* stream);
 
 /* Collector master's assembly (nodes/collector.py:193-236 after api/job_routes.py:126-130): frame i of n, a u8 frame
  * of frame_elems bytes at frames_dev[i] (a device array of n device pointers), goes to dst + i * frame_elems as

@@ -1,6 +1,8 @@
 """Per-tile time of a static-mode HTTP worker on cfg2 (7680x4320, 512 px tiles, padding 32, T0 sampler), split into
-its phases, for this package's worker (engine.WorkerJob + http_worker.HttpStaticWorker, the node's worker role) and for
-the reference's worker, both posting to the reference's master routes on 127.0.0.1 in this process.
+its phases, for this package's worker (engine.WorkerJob + http_worker.HttpStaticWorker) and for the reference's worker,
+all posting to the reference's master routes on 127.0.0.1 in this process.  This package's worker runs twice over the
+same tiles: once with the PNGs encoded on the GPU (WorkerJob.step_png, the node's worker role) and once PIL-encoded on
+the host (WorkerJob.step + http_worker.encode_png), so both encodes are timed on one card in one run.
 
 The master here only serves the queue: the job is created through the reference's own `init_static_job_batched` and
 nobody else pulls, so each worker gets every tile the queue holds.  The reference's worker takes seconds per tile at 8K
@@ -42,7 +44,8 @@ def start_job(env, job_id: str, n_tiles: int):
     env._call(env.mods["upscale.job_store"].init_static_job_batched(job_id, 1, n_tiles, [job_id]))
 
 
-def gpu_worker(env, url: str, img) -> dict:
+def gpu_worker(env, url: str, img, encode: str) -> dict:
+    """encode = "gpu": the node's worker role (WorkerJob.step_png); "pil": WorkerJob.step, PNGs from PIL on the host."""
     load_package()
     from comfyui_distributed_b200.denoise import T0Denoiser
     from comfyui_distributed_b200.engine import WorkerJob
@@ -51,23 +54,25 @@ def gpu_worker(env, url: str, img) -> dict:
     x = torch.from_numpy(img)
     warm = WorkerJob(x, T0Denoiser(SEED, DENOISE), TILE, TILE, PAD, BLUR, True)   # module loads, noise, work lists
     for t in range(len(warm.plan.tiles)):
-        warm.step(t)
+        warm.step_png(t) if encode == "gpu" else warm.step(t)                    # and the PNG layout check
     del warm
     torch.cuda.synchronize()
     t0 = time.perf_counter()
     job = WorkerJob(x, T0Denoiser(SEED, DENOISE), TILE, TILE, PAD, BLUR, True)
     setup = time.perf_counter() - t0
     n = len(job.plan.tiles)
-    start_job(env, "gpu", n)
-    w = HttpStaticWorker(url, "gpu", "gpu", PAD, [(t.x1, t.y1, t.ew, t.eh) for t in job.plan.tiles], 1)
+    job_id = "gpu-" + encode
+    start_job(env, job_id, n)
+    w = HttpStaticWorker(url, job_id, job_id, PAD, [(t.x1, t.y1, t.ew, t.eh) for t in job.plan.tiles], 1)
     t0 = time.perf_counter()
-    assert w.run(job.step)
+    assert w.run(job.step_png if encode == "gpu" else job.step)
     wall = time.perf_counter() - t0
     assert sorted(w.pulled) == list(range(n)), "the GPU worker did not get every tile"
     ms = lambda s: round(1e3 * s / n, 3)   # noqa: E731
     return {"tiles": n, "setup_ms": round(1e3 * setup, 1), "per_tile_ms": {
-        "device_step": round(job.times["device_ms"] / n, 3), "d2h": round(job.times["d2h_ms"] / n, 3),
-        "step_host_wall": ms(w.times["step_s"]), "png_encode": ms(w.times["encode_s"]), "post": ms(w.times["post_s"]),
+        "device_step": round(job.times["device_ms"] / n, 3), "gpu_png_encode": round(job.times["encode_ms"] / n, 3),
+        "d2h": round(job.times["d2h_ms"] / n, 3), "step_host_wall": ms(w.times["step_s"]),
+        "pil_png_encode": ms(w.times["encode_s"]), "post": ms(w.times["post_s"]),
         "heartbeat": ms(w.times["heartbeat_s"]), "tile_request": ms(w.times["request_s"]), "total_wall": ms(wall)},
         "uploads": w.chunks}
 
@@ -138,7 +143,8 @@ def main() -> int:
         env.sampler = ref_static_run.torch_t0
         url = f"http://127.0.0.1:{env.port}"
         res = {"card": card(), "cfg": f"{W}x{H} tile {TILE} padding {PAD} mask_blur {BLUR}, B=1, T0 sampler",
-               "gpu_worker": gpu_worker(env, url, img), "reference_worker": ref_worker(env, url, img, args.ref_tiles)}
+               "gpu_worker_gpu_png": gpu_worker(env, url, img, "gpu"), "gpu_worker_pil_png": gpu_worker(env, url, img, "pil"),
+               "reference_worker": ref_worker(env, url, img, args.ref_tiles)}
     finally:
         env.close()
     print(json.dumps(res, indent=1))
