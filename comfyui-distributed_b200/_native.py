@@ -16,7 +16,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libusdu_b200.so")
 
 # constants mirrored from include/usdu_b200.h (checked against the header in tests)
-ABI_VERSION = 16
+ABI_VERSION = 17
 ERR_INVALID = -1
 CANVAS_SLACK = 16
 PLAN_INFO_WORDS = 16
@@ -97,6 +97,7 @@ _SIGNATURES = {
     "usdu_png_encode_u8": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int64, c_void_p, c_int, c_void_p,
                                    c_int, POINTER(c_int64), c_void_p, c_void_p, c_void_p]),
     "usdu_gather_unpack_f32": (c_int, [c_void_p, c_int, c_int64, c_void_p, c_void_p]),
+    "usdu_b64_png_check": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p]),
     "usdu_t0_denoise": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_float, c_void_p]),
     "usdu_mask_scratch_bytes": (c_int64, [POINTER(c_int32), c_int]),
     "usdu_build_feather_masks": (c_int, [POINTER(c_int32), c_int, c_void_p, c_void_p, c_void_p]),
@@ -508,6 +509,30 @@ def png_decode_warps(max_row_bytes: int) -> int:
 def gather_unpack_f32(frame_ptrs_dev, n, frame_elems, dst_ptr, stream):
     """frame_ptrs_dev: device array of n u8 frame addresses; dst: device or pinned host memory (usdu_gather_unpack_f32)."""
     _check(lib().usdu_gather_unpack_f32(frame_ptrs_dev, n, frame_elems, dst_ptr, stream), "usdu_gather_unpack_f32")
+
+
+# usdu_b64_png_check's table (include/usdu_b200.h)
+B64_HEAD_WORDS = 24
+B64_MAX_CHUNKS = 4096
+B64_MAX_BLOCKS = 4096
+B64_PREFIX_BYTES = 4096
+B64_TABLE_WORDS = B64_HEAD_WORDS + 4 * B64_MAX_CHUNKS + 4 * B64_MAX_BLOCKS + B64_PREFIX_BYTES // 8
+B64_MAX_TEXT = (1 << 31) - 17                   # the largest text it takes
+(B64_CHUNKS_NONE, B64_CHUNKS_SHORT, B64_CHUNKS_PAST_END, B64_CHUNKS_AFTER_IDAT, B64_CHUNKS_IEND,
+ B64_CHUNKS_FULL) = range(6)
+(B64_BLOCKS_NONE, B64_BLOCKS_SHORT, B64_BLOCKS_ZLIB, B64_BLOCKS_COMPRESSED, B64_BLOCKS_LEN, B64_BLOCKS_FINAL,
+ B64_BLOCKS_FULL) = range(7)
+
+
+def b64_png_bytes(n: int) -> int:
+    """Device bytes usdu_b64_png_check writes the decoded text of n characters to."""
+    return 12 * ((n + 15) // 16)
+
+
+def b64_png_check(text_ptr, n, png_ptr, table_ptr, stream):
+    """text: n bytes in pinned host or device memory (16-byte aligned) -> decoded bytes at png_ptr and the verdict table
+    (B64_TABLE_WORDS int64, device) at table_ptr (usdu_b64_png_check)."""
+    _check(lib().usdu_b64_png_check(text_ptr, n, png_ptr, table_ptr, stream), "usdu_b64_png_check")
 
 
 def t0_denoise(tiles_ptr, noise_ptr, out_ptr, n, frame, omd, stream):

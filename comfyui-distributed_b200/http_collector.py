@@ -4,12 +4,18 @@ workers' images decoded and assembled on this GPU.
 
 The routes and the job state (multi_job_id -> asyncio.Queue, plus a lock) live on ComfyUI's server event loop, as in
 the reference; the master's prompt thread reaches them with `run_coroutine_threadsafe`.  The job_complete handler checks
-a POST in the reference's order and answers with its status codes and JSON bodies, but never decodes pixels: the base64
-text is decoded on the host with the reference's own call (`b64decode(validate=True)` fixes which texts are accepted),
-and the PNG is validated with http_master.parse_png, which keeps the bytes and the segment table of the filtered rows.
-The master uploads each drained batch of frames and decodes it on a side stream (http_master.PngDecoder) while it waits
-for more, and assembles the result with one usdu_gather_unpack_f32 launch that writes every worker frame, as k / 255,
-straight into the pinned host result in its final order.
+a POST in the reference's order and answers with its status codes and JSON bodies, but never decodes pixels.  With a
+CUDA device (DeviceChecks), the image's base64 text is decoded on the device and the decoded PNG's Adler-32 and filter
+bytes are checked there (csrc/usdu_b64.cu); the handler awaits the result without holding the loop, replays
+http_master.parse_png's structural walk over the chunk and block headers the device read out (check_png_tables), and
+queues the PNG as it lies on the device (DevicePng, a lease on a bounded DevicePool), on the device the job's master
+decodes on.  Without a device, when the buffers cannot be had (the pool's bound, or device or pinned memory the master's
+model holds), or for what the device tables do not settle (compressed blocks, more chunks or blocks than the table
+holds), the host path png_of_payload answers as the reference does (`b64decode(validate=True)`, then parse_png).  Both give every body the
+same answer.  The master decodes each drained batch of frames on a side stream (http_master.PngDecoder), from the
+device buffers or through a pinned upload, while it waits for more, and assembles the result with one
+usdu_gather_unpack_f32 launch that writes every worker frame, as k / 255, straight into the pinned host result in its
+final order.
 
 Differences from the reference (INTEGRATION.md, "A master for HTTP workers"):
 * images PIL would open but parse_png refuses answer the reference's decode-failure response (500, "Failed to decode
@@ -26,13 +32,18 @@ import asyncio
 import base64
 import binascii
 import os
+import struct
 import time
 import warnings
+import weakref
+import zlib
 from typing import Callable, Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 
-from .http_master import PngInfo, heartbeat_interval, heartbeat_timeout, parse_png
+from . import _native as nat
+from .http_master import (CHANNELS, PNG_MAX_ROW_BYTES, PNG_SIGNATURE, PngInfo, _IdatStream, heartbeat_interval,
+                          heartbeat_timeout, parse_png)
 
 JOB_INIT_GRACE_PERIOD = 10.0        # utils/constants.py:37: how long a POST waits for its job's queue
 GRACE_POLL = 0.05                   # job_routes.py:333
@@ -65,8 +76,13 @@ def field_errors(data: dict) -> List[str]:
     return errors
 
 
-def png_of_payload(image: str) -> Tuple[bytes, PngInfo]:
-    """The image field -> (PNG bytes, their validation), or ValueError with the reference's message."""
+NOT_BASE64 = "Field 'image' is not valid base64 PNG data."
+EMPTY_PNG = "Field 'image' decoded to empty PNG data."
+PNG_FAILED = "Failed to decode PNG image payload: "
+
+
+def payload_text(image: str) -> str:
+    """The image field -> its base64 text (after a data URL's header), or ValueError with the reference's message."""
     text = image.strip()
     if text.startswith("data:"):
         header, sep, body = text.partition(",")
@@ -75,17 +91,317 @@ def png_of_payload(image: str) -> Tuple[bytes, PngInfo]:
         if not header.lower().startswith("data:image/png;base64"):
             raise ValueError("Field 'image' must be a PNG data URL when using data:* format.")
         text = body
+    return text
+
+
+def png_of_payload(image: str) -> Tuple[bytes, PngInfo]:
+    """The image field -> (PNG bytes, their validation), or ValueError with the reference's message: the host path."""
+    text = payload_text(image)
     try:
         png = base64.b64decode(text, validate=True)
     except (binascii.Error, ValueError) as exc:
-        raise ValueError("Field 'image' is not valid base64 PNG data.") from exc
+        raise ValueError(NOT_BASE64) from exc
     if not png:
-        raise ValueError("Field 'image' decoded to empty PNG data.")
+        raise ValueError(EMPTY_PNG)
     try:
         info = parse_png(png)
     except Exception as exc:
-        raise ValueError(f"Failed to decode PNG image payload: {exc}") from exc
+        raise ValueError(f"{PNG_FAILED}{exc}") from exc
     return png, info
+
+
+# --------------------------------------------------------------------------------------
+# parse_png split: the device tables of usdu_b64_png_check, the structural walk here
+# --------------------------------------------------------------------------------------
+_CB = nat.B64_HEAD_WORDS
+_BB = _CB + 4 * nat.B64_MAX_CHUNKS
+_PB = _BB + 4 * nat.B64_MAX_BLOCKS
+
+
+class HostParse(Exception):
+    """The device tables do not settle this file (a compressed block, more chunks or blocks than the table holds, chunks
+    before IDAT past the fetched prefix): parse_png decides on the whole file."""
+
+
+def check_png_tables(tab: np.ndarray, m: int) -> PngInfo:
+    """parse_png over the m-byte PNG that usdu_b64_png_check decoded, from its table `tab` (int64): the walk over the
+    chunk and stored-block headers here, with parse_png's checks and reasons in its order; the Adler-32 and the largest
+    filter byte from the device.  -> the same PngInfo, or ValueError with parse_png's reason, or HostParse."""
+    head = tab[:_CB]
+    prefix = tab[_PB:].view(np.uint8)[:min(m, nat.B64_PREFIX_BYTES)].tobytes()
+    nc = int(head[4])
+    ch = tab[_CB: _CB + 4 * nc].reshape(-1, 4).tolist()
+    if m < 8 or prefix[:8] != PNG_SIGNATURE:
+        raise ValueError("not a PNG file")
+    pos, i = 8, 0
+    ihdr = None
+    idat: List[Tuple[int, int]] = []
+    while True:
+        if pos + 8 > m:
+            raise ValueError("truncated PNG (chunk header)")
+        if i == nc:
+            raise HostParse("chunk table full")
+        at, length, ctype, _ = ch[i]
+        i += 1
+        if at != pos:
+            raise HostParse("chunk table out of step")
+        ctype = int(ctype).to_bytes(4, "big")
+        body = pos + 8
+        if length > 0x7FFFFFFF or body + length + 4 > m:
+            raise ValueError(f"truncated PNG ({ctype!r} chunk runs past the end)")
+        if ihdr is None:
+            if ctype != b"IHDR" or length != 13:
+                raise ValueError("first chunk is not IHDR")
+        if not idat and ctype != b"IDAT":
+            if body + length + 4 > len(prefix):
+                raise HostParse("chunk before IDAT past the prefix")
+            crc, = struct.unpack_from(">I", prefix, body + length)
+            if zlib.crc32(prefix[pos + 4: body + length]) != crc:
+                raise ValueError(f"bad CRC in {ctype.decode('latin-1')}")
+        if ctype == b"IHDR":
+            if ihdr is not None:
+                raise ValueError("second IHDR")
+            W, H, depth, color, comp, filt, interlace = struct.unpack_from(">IIBBBBB", prefix, body)
+            if W == 0 or H == 0 or W > 0x7FFFFFFF or H > 0x7FFFFFFF:
+                raise ValueError("bad image size")
+            if depth != 8 or color not in CHANNELS:
+                raise ValueError(f"unsupported PNG: bit depth {depth}, colour type {color}")
+            if comp != 0 or filt != 0:
+                raise ValueError("unknown compression or filter method")
+            if interlace != 0:
+                raise ValueError("unsupported PNG: interlaced")
+            if W * CHANNELS[color] > PNG_MAX_ROW_BYTES:
+                raise ValueError(f"unsupported PNG: rows of {W * CHANNELS[color]} bytes (at most {PNG_MAX_ROW_BYTES})")
+            ihdr = (W, H, CHANNELS[color])
+        elif ctype == b"IDAT":
+            if idat and idat[-1][0] + idat[-1][1] + 4 != pos:
+                raise ValueError("IDAT chunks are not consecutive")
+            idat.append((body, length))
+        elif idat:
+            break
+        elif ctype == b"IEND":
+            raise ValueError("no IDAT chunk")
+        pos = body + length + 4
+    W, H, C = ihdr
+    raw_len = H * (1 + W * C)
+    st = _IdatStream(None, idat)
+    if st.size != int(head[8]):
+        raise HostParse("stream size out of step")
+    # _stored_segments
+    if st.size < 2:
+        raise ValueError("truncated deflate stream")
+    zh = int(head[7])
+    cmf, flg = zh & 0xFF, zh >> 8
+    if (cmf & 0x0F) != 8 or (cmf >> 4) > 7 or (cmf * 256 + flg) % 31 != 0 or (flg & 0x20):
+        raise ValueError("bad zlib header")
+    nb, code = int(head[9]), int(head[10])
+    bl = tab[_BB: _BB + 4 * nb].reshape(-1, 4).tolist()
+    pos, raw, segs, j = 2, 0, [], 0
+    while True:
+        if j == nb:
+            if code == nat.B64_BLOCKS_SHORT:
+                raise ValueError("truncated deflate stream")
+            raise HostParse("block table full")
+        at, packed, _, _ = bl[j]
+        j += 1
+        if at != pos:
+            raise HostParse("block table out of step")
+        hb = packed & 0xFF
+        if (hb >> 1) & 3 != 0:
+            raise HostParse("compressed block")
+        ln, nln = (packed >> 8) & 0xFFFF, (packed >> 24) & 0xFFFF
+        if ln ^ nln != 0xFFFF:
+            raise ValueError("stored block LEN/NLEN mismatch")
+        pos += 5
+        if pos + ln > st.size:
+            raise ValueError("truncated deflate stream")
+        for off, k in st.ranges(pos, ln):
+            use = min(k, raw_len - raw)
+            if use > 0:
+                segs.append((off, raw))
+            raw += use
+        pos += ln
+        if hb & 1:
+            break
+    if raw < raw_len:
+        raise ValueError("image data is truncated")
+    if pos + 4 > st.size:
+        raise ValueError("truncated deflate stream")
+    if code != nat.B64_BLOCKS_FINAL or int(head[15]) != pos or int(head[13]) < 0:
+        raise HostParse("device checks out of step")
+    if int(head[11]) != int(head[12]):
+        raise ValueError("bad Adler-32 of the image data")
+    trailer = [off + i for off, k in st.ranges(pos, 4) for i in range(k)]
+    info = PngInfo(W, H, C, segs, None, [(off - 8, ln) for off, ln in idat], trailer)
+    if int(head[13]) > 4:
+        raise ValueError("unrecognized data stream contents (filter type > 4)")
+    return info
+
+
+# --------------------------------------------------------------------------------------
+# the device path of the image checks
+# --------------------------------------------------------------------------------------
+POOL_BYTES = 4 << 30        # device bytes of decoded PNGs held at once: 81 4K RGB frames are about 2 GB
+WAIT_POLL = 0.0005          # s between polls of a CUDA event on the loop
+
+
+class DevicePool:
+    """The device buffers of decoded PNGs waiting in the collector queues, at most `limit` bytes at once.  A buffer
+    returns to the pool when its DevicePng is dropped (after the master decoded it, or with its job).  A request that
+    would pass the limit takes the host path."""
+
+    def __init__(self, limit: int = POOL_BYTES):
+        self.limit, self.used = int(limit), 0
+
+    def take(self, nbytes: int, device, stream):
+        import torch
+        if self.used + nbytes > self.limit:
+            return None
+        with torch.cuda.device(device), torch.cuda.stream(stream):
+            buf = torch.empty(nbytes, dtype=torch.uint8, device=device)
+        self.used += nbytes
+        return buf
+
+    def give(self, nbytes: int):
+        self.used -= nbytes
+
+
+class DevicePng:
+    """A decoded PNG on the device: buf[:size] (uint8), written once `ready` (a CUDA event) has completed.  len() is
+    its size; bytes(), slicing and == copy it to the host once (tests, a consumer on another device)."""
+    __slots__ = ("buf", "size", "ready", "_host", "__weakref__")
+
+    def __init__(self, buf, size: int, ready):
+        self.buf, self.size, self.ready, self._host = buf, int(size), ready, None
+
+    def __len__(self):
+        return self.size
+
+    def __bytes__(self):
+        if self._host is None:
+            self.ready.synchronize()
+            self._host = self.buf[:self.size].cpu().numpy().tobytes()
+        return self._host
+
+    def __getitem__(self, k):
+        return bytes(self)[k]
+
+    def __eq__(self, other):
+        if isinstance(other, DevicePng):
+            other = bytes(other)
+        if isinstance(other, (bytes, bytearray, memoryview)):
+            return bytes(self) == bytes(other)
+        return NotImplemented
+
+    __hash__ = None
+
+
+async def device_wait(event):
+    """Wait for a CUDA event without holding the event loop."""
+    while not event.query():
+        await asyncio.sleep(WAIT_POLL)
+
+
+class DeviceChecks:
+    """The image checks of job_complete on one device, on a stream of its own: usdu_b64_png_check, then the
+    structural walk on the host (check_png_tables).  One per device and process (device_checks())."""
+
+    def __init__(self, device, pool: Optional[DevicePool] = None):
+        import torch
+        self.device = torch.device(device)
+        with torch.cuda.device(self.device):
+            self.stream = torch.cuda.Stream(self.device)
+        self.pool = pool if pool is not None else DevicePool()
+        self.stats = {"device": 0, "host": 0}
+
+    def _buffers(self, n: int):
+        """-> (PNG buffer, pinned text, device table, pinned table) for an n-byte text, or None when they cannot all be
+        had: past the pool's bound, or out of device or pinned memory (the model the master runs may hold it)."""
+        import torch
+        nbytes = max(16, nat.b64_png_bytes(n))
+        try:
+            buf = self.pool.take(nbytes, self.device, self.stream)
+            if buf is None:
+                return None
+            weakref.finalize(buf, self.pool.give, nbytes)
+            pinned = torch.empty((n + 15) // 16 * 16 or 16, dtype=torch.uint8, pin_memory=True)
+            tab = torch.empty(nat.B64_TABLE_WORDS, dtype=torch.int64, pin_memory=True)
+            with torch.cuda.device(self.device), torch.cuda.stream(self.stream):
+                tab_dev = torch.empty(nat.B64_TABLE_WORDS, dtype=torch.int64, device=self.device)
+        except RuntimeError:                            # torch.OutOfMemoryError, or a failed pinned allocation
+            return None
+        return buf, pinned, tab_dev, tab
+
+    async def png_of_payload(self, image: str):
+        """png_of_payload with the base64 decode and the PNG's O(bytes) checks on the device: the same answer for
+        every field.  What the device cannot take (no buffers, a text of 2^31 bytes or more) or the tables do not
+        settle (HostParse) gets the host path's answer from png_of_payload itself.  -> (DevicePng or bytes, PngInfo)."""
+        import torch
+        text = payload_text(image)
+        try:
+            raw = text.encode("ascii")                  # b64decode refuses a str with other characters the same way
+        except UnicodeEncodeError as exc:
+            raise ValueError(NOT_BASE64) from exc
+        n = len(raw)
+        got = self._buffers(n) if n <= nat.B64_MAX_TEXT else None
+        if got is None:
+            self.stats["host"] += 1
+            return png_of_payload(image)
+        buf, pinned, tab_dev, tab = got
+        pinned.numpy()[:n] = np.frombuffer(raw, np.uint8)
+        del raw, got
+        with torch.cuda.device(self.device), torch.cuda.stream(self.stream):
+            nat.b64_png_check(pinned.data_ptr(), n, buf.data_ptr(), tab_dev.data_ptr(), self.stream.cuda_stream)
+            tab.copy_(tab_dev, non_blocking=True)
+            ready = torch.cuda.Event()
+            ready.record(self.stream)
+        await device_wait(ready)
+        del pinned, tab_dev
+        t = tab.numpy()
+        m = int(t[3])
+        if m < 0:
+            raise ValueError(NOT_BASE64)
+        if m == 0:
+            raise ValueError(EMPTY_PNG)
+        try:
+            info = check_png_tables(t, m)
+        except HostParse:
+            del buf
+            self.stats["host"] += 1
+            return png_of_payload(image)
+        except Exception as exc:
+            raise ValueError(f"{PNG_FAILED}{exc}") from exc
+        self.stats["device"] += 1
+        return DevicePng(buf, m, ready), info
+
+
+_checks: Dict = {}
+_cuda_ok: Optional[bool] = None
+
+
+def device_checks(device=None) -> Optional[DeviceChecks]:
+    """The DeviceChecks of `device` (a CUDA device; None: the current one) when this process has a CUDA device and the
+    library loads, else None (the host path).  job_complete asks for the device its job's master runs on."""
+    global _cuda_ok
+    if _cuda_ok is None:
+        try:
+            import torch
+            _cuda_ok = torch.cuda.is_available()
+            if _cuda_ok:
+                nat.lib()
+        except Exception:
+            _cuda_ok = False
+    if not _cuda_ok:
+        return None
+    import torch
+    dev = torch.device(device) if device is not None else torch.device("cuda")
+    if dev.type != "cuda":
+        dev = torch.device("cuda")
+    if dev.index is None:
+        dev = torch.device("cuda", torch.cuda.current_device())
+    if dev not in _checks:
+        _checks[dev] = DeviceChecks(dev)
+    return _checks[dev]
 
 
 def audio_of_payload(payload) -> Optional[dict]:
@@ -135,10 +451,12 @@ def audio_of_payload(payload) -> Optional[dict]:
 # --------------------------------------------------------------------------------------
 class CollectorStore:
     """The collector jobs of one server, touched only on its event loop.  A queue item is {"png", "info",
-    "worker_id", "image_index", "is_last", "audio"}: the PNG as posted (validated, not decoded)."""
+    "worker_id", "image_index", "is_last", "audio"}: the PNG as posted (validated, not decoded), as bytes or as a
+    DevicePng."""
 
     def __init__(self):
         self.jobs: Dict[str, asyncio.Queue] = {}
+        self.devices: Dict[str, object] = {}
         self._lock: Optional[asyncio.Lock] = None
 
     @property
@@ -147,10 +465,13 @@ class CollectorStore:
             self._lock = asyncio.Lock()
         return self._lock
 
-    async def prepare(self, multi_job_id):
+    async def prepare(self, multi_job_id, device=None):
+        """The job's queue; `device`: the CUDA device its master decodes on (job_complete checks its images there)."""
         async with self.lock:
             if multi_job_id not in self.jobs:
                 self.jobs[multi_job_id] = asyncio.Queue()
+            if device is not None:
+                self.devices[multi_job_id] = device
 
     async def put(self, multi_job_id, item: dict) -> bool:
         async with self.lock:
@@ -187,6 +508,7 @@ class CollectorStore:
     async def remove(self, multi_job_id):
         async with self.lock:
             self.jobs.pop(multi_job_id, None)
+            self.devices.pop(multi_job_id, None)
 
 
 # --------------------------------------------------------------------------------------
@@ -199,8 +521,9 @@ def _error(error, status=500):
     return web.json_response({"error": str(error)}, status=status)
 
 
-def make_handlers(store: CollectorStore, clock: Callable[[], float] = time.monotonic):
-    """The two route handlers over `store` -> {(method, path): handler}."""
+def make_handlers(store: CollectorStore, clock: Callable[[], float] = time.monotonic, checks=None):
+    """The two route handlers over `store` -> {(method, path): handler}.  `checks`: the DeviceChecks job_complete uses,
+    False for the host path, None for this process's (device_checks())."""
     from aiohttp import web
 
     async def prepare_job(request):
@@ -225,7 +548,11 @@ def make_handlers(store: CollectorStore, clock: Callable[[], float] = time.monot
             errors = field_errors(data)
             if errors:
                 return _error(errors, 400)
-            png, info = png_of_payload(data["image"])
+            dev = device_checks(store.devices.get(data["job_id"].strip())) if checks is None else checks
+            if dev:
+                png, info = await dev.png_of_payload(data["image"])
+            else:
+                png, info = png_of_payload(data["image"])
             audio = audio_of_payload(data.get("audio")) if data.get("audio") is not None else None
             item = {"png": png, "info": info, "worker_id": data["worker_id"].strip(),
                     "image_index": int(data["batch_idx"]), "is_last": data["is_last"], "audio": audio}
@@ -250,13 +577,13 @@ _loop = None
 _warned: set = set()
 
 
-def register(routes, store: CollectorStore = STORE, loop=None) -> set:
+def register(routes, store: CollectorStore = STORE, loop=None, checks=None) -> set:
     """Add the handlers to an aiohttp RouteTableDef (ComfyUI's PromptServer.instance.routes), skipping, with one warning
     each, every path another package already serves.  -> the (method, path) pairs this module serves."""
     global _loop
     taken = {(getattr(r, "method", None), getattr(r, "path", None)) for r in routes}
     served = set()
-    for (method, path), fn in make_handlers(store).items():
+    for (method, path), fn in make_handlers(store, checks=checks).items():
         if (method, path) in taken:
             if (method, path) not in _warned:
                 _warned.add((method, path))
@@ -298,6 +625,7 @@ def reset_for_tests():
     _served.clear()
     _loop = None
     STORE.jobs.clear()
+    STORE.devices.clear()
     STORE._lock = None
 
 
@@ -306,15 +634,17 @@ def reset_for_tests():
 # --------------------------------------------------------------------------------------
 class GpuFrames:
     """Each `add`ed batch of queue items is decoded on the side stream into one fresh device buffer, a 16-byte
-    aligned u8 [H, W, 3] slot per frame (item["frame"] = (buffer, offset)).  `assemble` writes the result."""
+    aligned u8 [H, W, 3] slot per frame (item["frame"] = (buffer, offset)).  `assemble` writes the result.
+    stats["device_frames"] counts the frames decoded from the route's device buffers, with no upload."""
 
     def __init__(self, device):
         from .http_master import PngDecoder
         self.device = device
         self.decoder = PngDecoder(device)
-        self.stats = {"upload_ms": 0.0, "decode_ms": 0.0, "assembly_ms": 0.0, "decode_launches": 0}
+        self.stats = {"upload_ms": 0.0, "decode_ms": 0.0, "assembly_ms": 0.0, "decode_launches": 0, "device_frames": 0}
 
     def add(self, items: Sequence[dict]):
+        """A PNG kept on this device (DevicePng, stored blocks) is decoded where it lies; any other is uploaded."""
         import torch
         if not items:
             return
@@ -324,10 +654,21 @@ class GpuFrames:
             cur += (it["info"].H * it["info"].W * 3 + 15) // 16 * 16
         with torch.cuda.device(self.device):
             buf = torch.empty(max(cur, 16), dtype=torch.uint8, device=self.device)
-        self.decoder.decode([(it["info"], it["png"], o) for it, o in zip(items, offs)], buf)
+        here = torch.device(self.device)
+        on_dev, up = [], []
+        for it, o in zip(items, offs):
+            png = it["png"]
+            if isinstance(png, DevicePng) and png.buf.device == here and it["info"].inflated is None:
+                on_dev.append((it["info"], png, o))
+            else:
+                up.append((it["info"], bytes(png), o))
+        for part, fn in ((up, self.decoder.decode), (on_dev, self.decoder.decode_device)):
+            if part:
+                fn(part, buf)
+                self.stats["decode_launches"] += 1
+        self.stats["device_frames"] += len(on_dev)
         for it, o in zip(items, offs):
             it["frame"] = (buf, o)
-        self.stats["decode_launches"] += 1
 
     def assemble(self, head, items: Sequence[dict], shape: Tuple[int, int, int], dtype):
         """-> CPU tensor [len(head) + len(items), *shape] of `dtype`: `head` (the master's frames, any device, or None)
@@ -392,11 +733,16 @@ class HttpCollectorMaster:
         from .nodes.collector import combine_audio
         empty = {"waveform": torch.zeros(1, 2, 1), "sample_rate": EMPTY_AUDIO_SAMPLE_RATE}
         job = self.multi_job_id
-        self._call(self.store.prepare(job))             # the queue exists before any local work (collector.py:261-268)
+        if self.frames is None:
+            dev = self.device if self.device is not None else \
+                images.device if images.is_cuda else torch.device("cuda", torch.cuda.current_device())
+        else:
+            dev = getattr(self.frames, "device", None)
+        # the queue exists before any local work (collector.py:261-268); the route checks images on the master's device
+        self._call(self.store.prepare(job, dev))
         try:
             if self.frames is None:
-                dev = images.device if images.is_cuda else torch.device("cuda", torch.cuda.current_device())
-                self.frames = GpuFrames(self.device if self.device is not None else dev)
+                self.frames = GpuFrames(dev)
             held, worker_audio = self._collect()
         finally:
             self._call(self.store.remove(job))

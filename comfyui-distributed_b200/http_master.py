@@ -702,6 +702,36 @@ class PngDecoder:
         self._events.append((e_up, e0, e1))
         self._keep_alive.append((host, dev, dst))
 
+    def decode_device(self, items: Sequence[Tuple[PngInfo, object, int]], dst):
+        """items: (info of stored blocks, http_collector.DevicePng on this device, byte offset of the frame's output in
+        `dst`): decoded where the PNGs lie, after each one's `ready` event; only the segment table is uploaded."""
+        import torch
+        from . import _native as nat
+        if not items:
+            return
+        base = min(png.buf.data_ptr() for _, png, _ in items)
+        segs, descs, max_row = [], [], 1
+        for info, png, off in items:
+            descs.append([len(segs), len(info.segs), info.H, info.W, info.C, off, 0, 0])
+            at = png.buf.data_ptr() - base
+            segs.extend((at + o, r) for o, r in info.segs)
+            max_row = max(max_row, info.W * info.C)
+        tabs = np.concatenate([np.asarray(segs, np.int64).reshape(-1), np.asarray(descs, np.int64).reshape(-1)])
+        host = torch.from_numpy(tabs).pin_memory()
+        with torch.cuda.device(self.device), torch.cuda.stream(self.side):
+            for _, png, _ in items:
+                self.side.wait_event(png.ready)
+            dev = torch.empty(tabs.size, dtype=torch.int64, device=self.device)
+            e_up, e0, e1 = (torch.cuda.Event(enable_timing=True) for _ in range(3))
+            e_up.record(self.side)
+            dev.copy_(host, non_blocking=True)
+            e0.record(self.side)
+            nat.png_decode_u8(base, dev.data_ptr(), len(segs), dev.data_ptr() + 16 * len(segs), len(descs), max_row,
+                              dst.data_ptr(), self.side.cuda_stream)
+            e1.record(self.side)
+        self._events.append((e_up, e0, e1))
+        self._keep_alive.append((host, dev, dst, [png for _, png, _ in items]))
+
     def times(self) -> Tuple[float, float]:
         """-> (upload ms, decode ms) over every batch so far; the side stream must have finished."""
         return (sum(a.elapsed_time(b) for a, b, _ in self._events),

@@ -35,7 +35,7 @@ extern "C" {
 #pragma GCC visibility push(default) /* the library itself is built with -fvisibility=hidden */
 #endif
 
-#define USDU_ABI_VERSION 16
+#define USDU_ABI_VERSION 17
 
 typedef enum usdu_status {
     USDU_OK = 0,
@@ -358,6 +358,47 @@ int usdu_png_encode_u8(const uint8_t* src_dev, int B, int H, int W, int C, const
  * (cudaHostAlloc); the latter is written through its device alias, so one launch performs the conversion and the
  * device-to-host transfer. */
 int usdu_gather_unpack_f32(const uint8_t* const* frames_dev, int n, int64_t frame_elems, float* dst, void* stream);
+
+/* Collector master's job_complete checks (api/job_routes.py:104-139): the base64 text of a posted image decoded, and
+ * the decoded PNG's O(bytes) checks, on the device; the host keeps the structural walk (http_collector.py).
+ * usdu_b64_png_check: text (16-byte aligned; device or pinned host memory, read in place) holds n bytes, the image
+ * field after its data-URL header; n < 2^31.  png_dev (device, 16-byte aligned) gets the decoded bytes and needs
+ * 12 * ceil(n / 16) bytes.  table_dev (device) gets USDU_B64_TABLE_WORDS int64:
+ *   head (USDU_B64_HEAD_WORDS): [0] 1 if a byte lies outside [A-Za-z0-9+/=]; [1] index of the first '=' (n if none);
+ *     [2] index of the last other byte + 1 (0 if none); [3] decoded length m when Python's
+ *     binascii.a2b_base64(text, strict_mode=True) (3.12) accepts the text, else -1 -- accepted exactly when [0] is 0,
+ *     no other byte follows a '=' ([2] <= [1]), the text does not start with '=' and, with d = [1] data characters and
+ *     p = n - d pads: d % 4 == 0, or d % 4 == 2 with p == 2, or d % 4 == 3 with p == 1; m = 3 * (d / 4) + (0, -, 1, 2)
+ *     [d % 4]; the trailing bits of a short quad are ignored;
+ *     [4] chunks recorded; [5] why the chunk walk stopped (USDU_B64_CHUNKS_*); [6] the first chunk's IHDR raw stream
+ *     bytes H * (1 + W * C) (-1 unless it reads as IHDR of length 13, 8-bit, colour type 0/2/4/6, W * C <=
+ *     USDU_PNG_MAX_ROW_BYTES); [7] the zlib header bytes CMF | FLG << 8 (-1 if the stream is shorter); [8] bytes of the
+ *     IDAT stream; [9] stored blocks recorded; [10] why the block walk stopped (USDU_B64_BLOCKS_*); [11] the 4 bytes
+ *     after the final block, big-endian (-1 if the stream is shorter); [12] Adler-32 of the stored blocks' data (-1
+ *     unless the walk reached the final block); [13] the largest filter byte over the rows of [6] (-1 unless the blocks
+ *     hold that many bytes); [14] data bytes of the recorded blocks; [15] stream position after the final block;
+ *     [16] entry of the first IDAT chunk; [17] IDAT chunks;
+ *   USDU_B64_MAX_CHUNKS chunk entries of 4 words: file offset, data length, type (big-endian), IDAT stream start (-1);
+ *   USDU_B64_MAX_BLOCKS block entries of 4 words: stream offset of the block header, BFINAL/BTYPE byte | LEN << 8 |
+ *     NLEN << 24, offset of its data in the concatenated data of the blocks, Adler partials (s1 | s2 << 32);
+ *   the file's first min(m, USDU_B64_PREFIX_BYTES) bytes.
+ * The chunk walk goes from byte 8 through consecutive chunk headers, as http_master.parse_png does, and stops after
+ * the first chunk that is not IDAT following an IDAT, after an IEND before any IDAT, after a chunk whose length exceeds
+ * 2^31 - 1 or which runs past the end, when the next header does not fit, or at the table's end.  When it stopped
+ * after IDATs, the block walk follows the zlib stream of stored blocks through the IDAT chunks until the final block, a
+ * compressed block, a LEN/NLEN mismatch, a block or header past the stream's end, or the table's end.  Four launches on
+ * `stream`, no host synchronisation. */
+#define USDU_B64_HEAD_WORDS 24
+#define USDU_B64_MAX_CHUNKS 4096
+#define USDU_B64_MAX_BLOCKS 4096
+#define USDU_B64_PREFIX_BYTES 4096
+#define USDU_B64_TABLE_WORDS \
+    (USDU_B64_HEAD_WORDS + 4 * USDU_B64_MAX_CHUNKS + 4 * USDU_B64_MAX_BLOCKS + USDU_B64_PREFIX_BYTES / 8)
+enum { USDU_B64_CHUNKS_NONE = 0, USDU_B64_CHUNKS_SHORT = 1, USDU_B64_CHUNKS_PAST_END = 2, USDU_B64_CHUNKS_AFTER_IDAT = 3,
+       USDU_B64_CHUNKS_IEND = 4, USDU_B64_CHUNKS_FULL = 5 };
+enum { USDU_B64_BLOCKS_NONE = 0, USDU_B64_BLOCKS_SHORT = 1, USDU_B64_BLOCKS_ZLIB = 2, USDU_B64_BLOCKS_COMPRESSED = 3,
+       USDU_B64_BLOCKS_LEN = 4, USDU_B64_BLOCKS_FINAL = 5, USDU_B64_BLOCKS_FULL = 6 };
+int usdu_b64_png_check(const char* text, int64_t n, uint8_t* png_dev, int64_t* table_dev, void* stream);
 
 /* TEST DOUBLE, not part of the reference path: the deterministic T0 sampler stand-in used by the
  * parity tests and bench.py (BASELINE.md section 3) as one fused pass,
