@@ -16,7 +16,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libusdu_b200.so")
 
 # constants mirrored from include/usdu_b200.h (checked against the header in tests)
-ABI_VERSION = 17
+ABI_VERSION = 18
 ERR_INVALID = -1
 CANVAS_SLACK = 16
 PLAN_INFO_WORDS = 16
@@ -94,6 +94,7 @@ _SIGNATURES = {
     "usdu_png_base64_u8": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "usdu_png_decode_u8": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "usdu_png_decode_warps": (c_int, [c_int]),
+    "usdu_png_decode_general_u8": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "usdu_png_encode_u8": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int64, c_void_p, c_int, c_void_p,
                                    c_int, POINTER(c_int64), c_void_p, c_void_p, c_void_p]),
     "usdu_gather_unpack_f32": (c_int, [c_void_p, c_int, c_int64, c_void_p, c_void_p]),
@@ -483,6 +484,16 @@ PNG_MAX_ROW_BYTES = 65536      # 16,384 px (ComfyUI's MAX_RESOLUTION) at 4 chann
 def png_decode_u8(src_ptr, segs_ptr, n_segs, descs_ptr, n, max_row_bytes, dst_ptr, stream):
     _check(lib().usdu_png_decode_u8(src_ptr, segs_ptr, n_segs, descs_ptr, n, max_row_bytes, dst_ptr, stream),
            "usdu_png_decode_u8")
+
+
+PNG_GENERAL_DESC_WORDS = 16
+
+
+def png_decode_general_u8(src_ptr, descs_ptr, n, max_row_bytes, dst_ptr, stream):
+    """n pass descriptors (PNG_GENERAL_DESC_WORDS int64, device) over src -> u8 RGB frames in dst
+    (usdu_png_decode_general_u8)."""
+    _check(lib().usdu_png_decode_general_u8(src_ptr, descs_ptr, n, max_row_bytes, dst_ptr, stream),
+           "usdu_png_decode_general_u8")
 
 
 def png_encode_scratch_bytes(B: int, H: int, W: int) -> int:

@@ -150,6 +150,134 @@ __global__ void __launch_bounds__(kDecThreads) png_decode_kernel(const uint8_t* 
     }
 }
 
+// The general entry: a PNG of any colour type and bit depth, interlaced or not, its filtered stream R inflated on the
+// host (http_master.parse_png_general) and uploaded whole.  One CTA per (frame, pass): a non-interlaced frame is one
+// pass; Adam7's seven passes are independent PNG sub-images that scatter to (y0 + i*dy, x0 + j*dx).  The same chunked
+// wavefront, on PNG filter units of bpp = max(1, depth*C/8) bytes: a lane owns one unit (a pixel at depth >= 8, one
+// byte of 8/depth pixels below), a chunk is 32 units.  The store step converts as PIL's convert("RGB"): sub-byte grey
+// scaled to 0..255, 16-bit grey clipped to 255 (PIL's I;16), other 16-bit samples by their high byte, palette indices
+// looked up in a 256-entry table (entries past the PLTE's are zero), alpha dropped.
+__global__ void __launch_bounds__(kDecThreads) png_decode_general_kernel(const uint8_t* __restrict__ src,
+                                                                         const int64_t* __restrict__ descs,
+                                                                         uint8_t* __restrict__ dst) {
+    extern __shared__ __align__(16) uint8_t ring[];
+    __shared__ int prog[kDecWarps];
+    const int64_t* d = descs + (int64_t)blockIdx.x * USDU_PNG_GENERAL_DESC_WORDS;
+    const uint8_t* R = src + d[0];
+    const int W = (int)d[1], H = (int)d[2];                            // the pass's columns and rows
+    const int x0 = (int)d[3], y0 = (int)d[4], dx = (int)d[5], dy = (int)d[6];
+    const int64_t pitch = d[7];                                         // the frame's width
+    const int color = (int)d[8], depth = (int)d[9];
+    uint8_t* out = dst + d[10];
+    const uint8_t* pal = src + d[11];
+    const int C = color == 2 ? 3 : color == 4 ? 2 : color == 6 ? 4 : 1;
+    const int bpp = max(1, depth * C / 8);
+    const int n = (int)(((int64_t)W * depth * C + 7) / 8);             // filtered bytes of a row
+    const int units = (n + bpp - 1) / bpp;
+    const int nch = (units + kChunk - 1) / kChunk;
+    const int D = blockDim.x >> 5;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (threadIdx.x < D) prog[threadIdx.x] = 0;
+    __syncthreads();
+
+    uint8_t* mine = ring + warp * n;
+    for (int r = warp; r < H; r += D) {
+        const uint8_t* above = r > 0 ? ring + ((r - 1) % D) * n : nullptr;
+        const int* prog_above = &prog[(r - 1 + D) % D];
+        const int* prog_next = &prog[(warp + 1) % D];
+        const uint8_t* row = R + (int64_t)r * (n + 1);
+        const uint32_t filt = __shfl_sync(0xffffffffu, lane == 0 ? (uint32_t)row[0] : 0u, 0);
+        uint32_t carry[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+        for (int k = 0; k < nch; ++k) {
+            const int u = k * kChunk + lane;
+            const int cnt = min(kChunk, units - k * kChunk);
+            if (r >= D) wait_progress(prog_next, (r - D + 1) * nch + min(k + 2, nch));
+            if (r > 0 && (filt >= 2)) wait_progress(prog_above, (r - 1) * nch + k + 1);
+            uint32_t v[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+            if (lane < cnt) {
+#pragma unroll
+                for (int c = 0; c < 8; ++c)
+                    if (c < bpp) v[c] = row[1 + u * bpp + c];
+            }
+            if (filt == 1) {                                            // Sub: inclusive scan per unit byte
+#pragma unroll
+                for (int c = 0; c < 8; ++c) {
+                    if (c >= bpp) break;                                // bpp is uniform over the warp
+                    uint32_t s = v[c];
+#pragma unroll
+                    for (int o = 1; o < 32; o <<= 1) {
+                        const uint32_t t = __shfl_up_sync(0xffffffffu, s, o);
+                        if (lane >= o) s += t;
+                    }
+                    v[c] = (s + carry[c]) & 0xffu;
+                    carry[c] = __shfl_sync(0xffffffffu, v[c], cnt - 1);
+                }
+            } else if (filt == 2 && lane < cnt && r > 0) {              // Up
+#pragma unroll
+                for (int c = 0; c < 8; ++c)
+                    if (c < bpp) v[c] = (v[c] + above[u * bpp + c]) & 0xffu;
+            }
+            if (lane < cnt) {
+#pragma unroll
+                for (int c = 0; c < 8; ++c)
+                    if (c < bpp) mine[u * bpp + c] = (uint8_t)v[c];
+            }
+            __syncwarp();
+            if (filt >= 3 && lane < bpp) {                              // Avg, Paeth: serial per unit byte, in place
+                const int c = lane;
+                uint32_t left = k > 0 ? mine[(k * kChunk - 1) * bpp + c] : 0u;
+                uint32_t ul = (k > 0 && r > 0) ? above[(k * kChunk - 1) * bpp + c] : 0u;
+                for (int i = 0; i < cnt; ++i) {
+                    const int o = (k * kChunk + i) * bpp + c;
+                    const uint32_t up = r > 0 ? above[o] : 0u;
+                    const uint32_t f = mine[o];
+                    const uint32_t pred = filt == 3 ? ((left + up) >> 1) : paeth(left, up, ul);
+                    left = (f + pred) & 0xffu;
+                    mine[o] = (uint8_t)left;
+                    ul = up;
+                }
+            }
+            __syncwarp();
+            if (lane < cnt) {                                           // convert("RGB") and store
+                uint8_t* q = out + ((int64_t)(y0 + r * dy) * pitch + x0) * 3;
+                if (depth >= 8) {
+                    const uint8_t* p = mine + u * bpp;
+                    const int s = depth >> 3;                           // bytes per sample
+                    uint32_t c0, c1, c2;
+                    if (color == 3) {
+                        c0 = pal[3 * p[0]], c1 = pal[3 * p[0] + 1], c2 = pal[3 * p[0] + 2];
+                    } else if (color == 2 || color == 6) {
+                        c0 = p[0], c1 = p[s], c2 = p[2 * s];
+                    } else if (color == 0 && depth == 16) {
+                        c0 = c1 = c2 = min(((uint32_t)p[0] << 8) | p[1], 255u);
+                    } else {
+                        c0 = c1 = c2 = p[0];
+                    }
+                    uint8_t* o = q + (int64_t)u * dx * 3;
+                    o[0] = (uint8_t)c0, o[1] = (uint8_t)c1, o[2] = (uint8_t)c2;
+                } else {                                                // 8 / depth pixels in this byte
+                    const uint32_t b = mine[u];
+                    const int per = 8 / depth, mask = (1 << depth) - 1, scale = 255 / mask;
+                    for (int i = 0; i < per; ++i) {
+                        const int x = u * per + i;
+                        if (x >= W) break;                              // the row's padding bits
+                        const uint32_t sv = (b >> (8 - depth * (i + 1))) & mask;
+                        uint8_t* o = q + (int64_t)x * dx * 3;
+                        if (color == 3) {
+                            o[0] = pal[3 * sv], o[1] = pal[3 * sv + 1], o[2] = pal[3 * sv + 2];
+                        } else {
+                            o[0] = o[1] = o[2] = (uint8_t)(sv * scale);
+                        }
+                    }
+                }
+            }
+            __threadfence_block();
+            __syncwarp();
+            if (lane == 0) *reinterpret_cast<volatile int*>(&prog[warp]) = r * nch + k + 1;
+        }
+    }
+}
+
 // frame i of n: dst[i * frame_elems + e] = frames[i][e] / 255 (dequant_u8_fast, bit-identical to __fdiv_rn).  Each
 // thread writes 4 consecutive floats with one 16-byte store, from the frame's first 16-byte-aligned output element on
 // (its `head` elements before that are written singly), so a dst in mapped host memory gets whole 128-byte lines.
@@ -176,16 +304,16 @@ __global__ void __launch_bounds__(kThreads) gather_unpack_kernel(const uint8_t* 
     }
 }
 
-int decode_warps(int max_row_bytes, int* warps) {
+int decode_warps(const void* kernel, const char* what, int max_row_bytes, int* warps) {
     USDU_REQUIRE(max_row_bytes >= 1 && max_row_bytes <= USDU_PNG_MAX_ROW_BYTES,
-                 "usdu_png_decode_u8: row bytes %d outside [1, %d]", max_row_bytes, USDU_PNG_MAX_ROW_BYTES);
+                 "%s: row bytes %d outside [1, %d]", what, max_row_bytes, USDU_PNG_MAX_ROW_BYTES);
     int dev = 0, optin = 0;
     USDU_CUDA(cudaGetDevice(&dev));
     USDU_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
     cudaFuncAttributes a;
-    USDU_CUDA(cudaFuncGetAttributes(&a, (const void*)png_decode_kernel));
+    USDU_CUDA(cudaFuncGetAttributes(&a, kernel));
     const int64_t fit = ((int64_t)optin - (int64_t)a.sharedSizeBytes) / max_row_bytes;
-    USDU_REQUIRE(fit >= kDecMinWarps, "usdu_png_decode_u8: %d-byte rows leave room for %lld ring rows (need %d)",
+    USDU_REQUIRE(fit >= kDecMinWarps, "%s: %d-byte rows leave room for %lld ring rows (need %d)", what,
                  max_row_bytes, (long long)fit, kDecMinWarps);
     *warps = fit < kDecWarps ? (int)fit : kDecWarps;
     return USDU_OK;
@@ -200,7 +328,7 @@ extern "C" {
 
 int usdu_png_decode_warps(int max_row_bytes) {
     int warps = 0;
-    const int r = decode_warps(max_row_bytes, &warps);
+    const int r = decode_warps((const void*)png_decode_kernel, "usdu_png_decode_u8", max_row_bytes, &warps);
     return r != USDU_OK ? r : warps;
 }
 
@@ -211,12 +339,28 @@ int usdu_png_decode_u8(const uint8_t* src_dev, const int64_t* segs_dev, int64_t 
     USDU_REQUIRE(src_dev && segs_dev && descs_dev && dst_dev, "usdu_png_decode_u8: null pointer");
     USDU_REQUIRE(n_segs >= 1, "usdu_png_decode_u8: no segments");
     int warps = 0;
-    int r = decode_warps(max_row_bytes, &warps);
+    int r = decode_warps((const void*)png_decode_kernel, "usdu_png_decode_u8", max_row_bytes, &warps);
     if (r != USDU_OK) return r;
     const size_t smem = (size_t)warps * (size_t)max_row_bytes;
     r = raise_smem_limit((const void*)png_decode_kernel, smem);
     if (r != USDU_OK) return r;
     png_decode_kernel<<<n, warps * 32, smem, (cudaStream_t)stream>>>(src_dev, segs_dev, n_segs, descs_dev, dst_dev);
+    USDU_CUDA(cudaGetLastError());
+    return USDU_OK;
+}
+
+int usdu_png_decode_general_u8(const uint8_t* src_dev, const int64_t* descs_dev, int n, int max_row_bytes,
+                               uint8_t* dst_dev, void* stream) {
+    USDU_REQUIRE(n >= 0, "usdu_png_decode_general_u8: %d passes", n);
+    if (n == 0) return USDU_OK;
+    USDU_REQUIRE(src_dev && descs_dev && dst_dev, "usdu_png_decode_general_u8: null pointer");
+    int warps = 0;
+    int r = decode_warps((const void*)png_decode_general_kernel, "usdu_png_decode_general_u8", max_row_bytes, &warps);
+    if (r != USDU_OK) return r;
+    const size_t smem = (size_t)warps * (size_t)max_row_bytes;
+    r = raise_smem_limit((const void*)png_decode_general_kernel, smem);
+    if (r != USDU_OK) return r;
+    png_decode_general_kernel<<<n, warps * 32, smem, (cudaStream_t)stream>>>(src_dev, descs_dev, dst_dev);
     USDU_CUDA(cudaGetLastError());
     return USDU_OK;
 }

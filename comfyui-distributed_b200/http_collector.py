@@ -11,16 +11,18 @@ http_master.parse_png's structural walk over the chunk and block headers the dev
 queues the PNG as it lies on the device (DevicePng, a lease on a bounded DevicePool), on the device the job's master
 decodes on.  Without a device, when the buffers cannot be had (the pool's bound, or device or pinned memory the master's
 model holds), or for what the device tables do not settle (compressed blocks, more chunks or blocks than the table
-holds), the host path png_of_payload answers as the reference does (`b64decode(validate=True)`, then parse_png).  Both give every body the
-same answer.  The master decodes each drained batch of frames on a side stream (http_master.PngDecoder), from the
+holds), the host path png_of_payload answers as the reference does (`b64decode(validate=True)`, then parse_png).  A
+palette, 1/2/4/16-bit or interlaced PNG, which parse_png refuses for its IHDR, is validated and inflated on the host by
+http_master.parse_png_general (the device path hands it the decoded bytes) and decoded with usdu_png_decode_general_u8.
+Both paths give every body the same answer.  The master decodes each drained batch of frames on a side stream (http_master.PngDecoder), from the
 device buffers or through a pinned upload, while it waits for more, and assembles the result with one
 usdu_gather_unpack_f32 launch that writes every worker frame, as k / 255, straight into the pinned host result in its
 final order.
 
 Differences from the reference (INTEGRATION.md, "A master for HTTP workers"):
-* images PIL would open but parse_png refuses answer the reference's decode-failure response (500, "Failed to decode
-  PNG image payload: ..."): palette, 16-bit and interlaced PNGs, PNGs with rows over PNG_MAX_ROW_BYTES (16,384 RGBA
-  pixels), and other formats PIL detects (JPEG, BMP, ...).  Neither worker sends any of them;
+* images PIL would open but this module refuses answer the reference's decode-failure response (500, "Failed to
+  decode PNG image payload: ..."): PNGs with filtered rows over PNG_MAX_ROW_BYTES (16,384 8-bit RGBA pixels) and other
+  formats PIL detects (JPEG, BMP, ...).  Neither worker sends any of them;
 * no busy-probe of missing workers (collector.py:374-411 reads the orchestrator's gpu_config.json), and the worker
   timeout is COMFYUI_HEARTBEAT_TIMEOUT (default 60 s), not the config file's setting;
 * delegate-only mode comes from the node's hidden input only, not from the config file;
@@ -42,8 +44,8 @@ from typing import Callable, Dict, List, Optional, Sequence, Tuple
 import numpy as np
 
 from . import _native as nat
-from .http_master import (CHANNELS, PNG_MAX_ROW_BYTES, PNG_SIGNATURE, PngInfo, _IdatStream, heartbeat_interval,
-                          heartbeat_timeout, parse_png)
+from .http_master import (CHANNELS, PNG_MAX_ROW_BYTES, PNG_SIGNATURE, PngInfo, UnsupportedPng, _IdatStream,
+                          heartbeat_interval, heartbeat_timeout, parse_png, parse_png_any, parse_png_general)
 
 JOB_INIT_GRACE_PERIOD = 10.0        # utils/constants.py:37: how long a POST waits for its job's queue
 GRACE_POLL = 0.05                   # job_routes.py:333
@@ -95,7 +97,8 @@ def payload_text(image: str) -> str:
 
 
 def png_of_payload(image: str) -> Tuple[bytes, PngInfo]:
-    """The image field -> (PNG bytes, their validation), or ValueError with the reference's message: the host path."""
+    """The image field -> (PNG bytes, their validation: PngInfo, or PngGeneral for a palette, 1/2/4/16-bit or
+    interlaced PNG), or ValueError with the reference's message: the host path."""
     text = payload_text(image)
     try:
         png = base64.b64decode(text, validate=True)
@@ -104,7 +107,7 @@ def png_of_payload(image: str) -> Tuple[bytes, PngInfo]:
     if not png:
         raise ValueError(EMPTY_PNG)
     try:
-        info = parse_png(png)
+        info = parse_png_any(png)
     except Exception as exc:
         raise ValueError(f"{PNG_FAILED}{exc}") from exc
     return png, info
@@ -126,7 +129,8 @@ class HostParse(Exception):
 def check_png_tables(tab: np.ndarray, m: int) -> PngInfo:
     """parse_png over the m-byte PNG that usdu_b64_png_check decoded, from its table `tab` (int64): the walk over the
     chunk and stored-block headers here, with parse_png's checks and reasons in its order; the Adler-32 and the largest
-    filter byte from the device.  -> the same PngInfo, or ValueError with parse_png's reason, or HostParse."""
+    filter byte from the device.  -> the same PngInfo, or ValueError with parse_png's reason (UnsupportedPng where
+    parse_png raises it), or HostParse."""
     head = tab[:_CB]
     prefix = tab[_PB:].view(np.uint8)[:min(m, nat.B64_PREFIX_BYTES)].tobytes()
     nc = int(head[4])
@@ -165,11 +169,11 @@ def check_png_tables(tab: np.ndarray, m: int) -> PngInfo:
             if W == 0 or H == 0 or W > 0x7FFFFFFF or H > 0x7FFFFFFF:
                 raise ValueError("bad image size")
             if depth != 8 or color not in CHANNELS:
-                raise ValueError(f"unsupported PNG: bit depth {depth}, colour type {color}")
+                raise UnsupportedPng(f"unsupported PNG: bit depth {depth}, colour type {color}")
             if comp != 0 or filt != 0:
                 raise ValueError("unknown compression or filter method")
             if interlace != 0:
-                raise ValueError("unsupported PNG: interlaced")
+                raise UnsupportedPng("unsupported PNG: interlaced")
             if W * CHANNELS[color] > PNG_MAX_ROW_BYTES:
                 raise ValueError(f"unsupported PNG: rows of {W * CHANNELS[color]} bytes (at most {PNG_MAX_ROW_BYTES})")
             ihdr = (W, H, CHANNELS[color])
@@ -312,7 +316,7 @@ class DeviceChecks:
         with torch.cuda.device(self.device):
             self.stream = torch.cuda.Stream(self.device)
         self.pool = pool if pool is not None else DevicePool()
-        self.stats = {"device": 0, "host": 0}
+        self.stats = {"device": 0, "host": 0, "general": 0}
 
     def _buffers(self, n: int):
         """-> (PNG buffer, pinned text, device table, pinned table) for an n-byte text, or None when they cannot all be
@@ -369,6 +373,16 @@ class DeviceChecks:
             del buf
             self.stats["host"] += 1
             return png_of_payload(image)
+        except UnsupportedPng:
+            # palette, 1/2/4/16-bit or interlaced: parse_png_general inflates the decoded bytes, off the event loop
+            png = bytes(DevicePng(buf, m, ready))
+            del buf
+            self.stats["general"] += 1
+            try:
+                info = await asyncio.get_running_loop().run_in_executor(None, parse_png_general, png)
+            except Exception as exc:
+                raise ValueError(f"{PNG_FAILED}{exc}") from exc
+            return png, info
         except Exception as exc:
             raise ValueError(f"{PNG_FAILED}{exc}") from exc
         self.stats["device"] += 1
@@ -644,7 +658,8 @@ class GpuFrames:
         self.stats = {"upload_ms": 0.0, "decode_ms": 0.0, "assembly_ms": 0.0, "decode_launches": 0, "device_frames": 0}
 
     def add(self, items: Sequence[dict]):
-        """A PNG kept on this device (DevicePng, stored blocks) is decoded where it lies; any other is uploaded."""
+        """A PNG kept on this device (DevicePng, stored blocks) is decoded where it lies; any other is uploaded (a
+        PngGeneral's filtered stream, to usdu_png_decode_general_u8)."""
         import torch
         if not items:
             return
@@ -658,14 +673,15 @@ class GpuFrames:
         on_dev, up = [], []
         for it, o in zip(items, offs):
             png = it["png"]
-            if isinstance(png, DevicePng) and png.buf.device == here and it["info"].inflated is None:
+            if isinstance(png, DevicePng) and png.buf.device == here and isinstance(it["info"], PngInfo) \
+                    and it["info"].inflated is None:
                 on_dev.append((it["info"], png, o))
             else:
                 up.append((it["info"], bytes(png), o))
-        for part, fn in ((up, self.decoder.decode), (on_dev, self.decoder.decode_device)):
-            if part:
-                fn(part, buf)
-                self.stats["decode_launches"] += 1
+        self.stats["decode_launches"] += self.decoder.decode(up, buf)
+        if on_dev:
+            self.decoder.decode_device(on_dev, buf)
+            self.stats["decode_launches"] += 1
         self.stats["device_frames"] += len(on_dev)
         for it, o in zip(items, offs):
             it["frame"] = (buf, o)

@@ -5,14 +5,15 @@ the final composite (upscale/modes/static.py:371-570) on this GPU.
 The routes and the job store live on ComfyUI's server event loop, as in the reference; the master's prompt thread
 reaches them with `run_coroutine_threadsafe`.  A route handler never decodes pixels: it validates each posted PNG on the
 host (`parse_png`, which refuses what PIL's open().convert("RGB") refuses) and keeps the raw bytes, the segment table of
-the filtered stream inside them and the tile's metadata.  The master uploads each drained batch of tiles and decodes it
-on a side stream (csrc/usdu_png_decode.cu) while it waits for more, and composites all kept worker tiles in the
-reference's order with the existing blend kernels.
+the filtered stream inside them and the tile's metadata.  A palette, 1/2/4/16-bit or interlaced PNG, which parse_png
+refuses, is validated and inflated by `parse_png_general` instead, and its filtered stream kept.  The master uploads each
+drained batch of tiles and decodes it on a side stream (csrc/usdu_png_decode.cu) while it waits for more, and
+composites all kept worker tiles in the reference's order with the existing blend kernels.
 
 Differences from the reference (INTEGRATION.md, "A master for HTTP workers"):
 * no "busy" probe of a timed-out worker (job_timeout.py:82-105 reads the orchestrator's gpu_config.json): a worker whose
   heartbeat is older than COMFYUI_HEARTBEAT_TIMEOUT has its incomplete tiles re-queued;
-* palette, 16-bit and interlaced PNGs answer 400 (neither worker produces them);
+* PNGs with filtered rows over PNG_MAX_ROW_BYTES answer 400;
 * x, y, extracted_width and extracted_height must equal the plan's window of tile_idx, and the PNG must be at the tile's
   processing size, else 400;
 * a job is cleaned up in a `finally` around the whole master run, including an interrupt before the collect phase.
@@ -71,12 +72,44 @@ class PngInfo:
         return self.H * (1 + self.W * self.C)
 
 
+class UnsupportedPng(ValueError):
+    """parse_png's refusal of a bit depth, colour type or interlace method it does not take: parse_png_general decides
+    such a file."""
+
+
 def parse_png(data: bytes) -> PngInfo:
     """Validate `data` as PIL's open().convert("RGB") would read it and return its segment table.  ValueError with the
-    reason otherwise.  Checks: signature; IHDR (8-bit, colour type 0/2/4/6, no interlace); chunk bounds; the CRC-32 of
-    every chunk before the first IDAT (PIL checks those, not IDAT's or later ones); the zlib header; the stored-block
-    LEN/NLEN chain (any compressed block: the stream is inflated with zlib); the Adler-32; the IDAT length against the
-    image size; every filter byte <= 4; rows of at most PNG_MAX_ROW_BYTES (what the decode kernel takes)."""
+    reason otherwise (UnsupportedPng for the IHDR's depth, colour type or interlace).  Checks: signature; IHDR (8-bit,
+    colour type 0/2/4/6, no interlace); chunk bounds; the CRC-32 of every chunk before the first IDAT (PIL checks those,
+    not IDAT's or later ones); the zlib header; the stored-block LEN/NLEN chain (any compressed block: the stream is
+    inflated with zlib); the Adler-32; the IDAT length against the image size; every filter byte <= 4; rows of at most
+    PNG_MAX_ROW_BYTES (what the decode kernel takes)."""
+    (W, H, C), idat, _ = _walk_chunks(data, _ihdr_8bit)
+    raw_len = H * (1 + W * C)
+    stream = _IdatStream(data, idat)
+    segs, inflated, trailer = _stored_segments(stream, raw_len)
+    info = PngInfo(W, H, C, segs, inflated, [(off - 8, ln) for off, ln in idat], trailer)
+    _check_filters(info, data)
+    return info
+
+
+def _ihdr_8bit(W, H, depth, color, comp, filt, interlace):
+    if depth != 8 or color not in CHANNELS:
+        raise UnsupportedPng(f"unsupported PNG: bit depth {depth}, colour type {color}")
+    if comp != 0 or filt != 0:
+        raise ValueError("unknown compression or filter method")
+    if interlace != 0:
+        raise UnsupportedPng("unsupported PNG: interlaced")
+    if W * CHANNELS[color] > PNG_MAX_ROW_BYTES:
+        raise ValueError(f"unsupported PNG: rows of {W * CHANNELS[color]} bytes (at most {PNG_MAX_ROW_BYTES})")
+    return W, H, CHANNELS[color]
+
+
+def _walk_chunks(data: bytes, on_ihdr, keep=()):
+    """The chunk walk both parses share: signature, chunk bounds, IHDR first (its fields go to `on_ihdr`, which raises
+    or returns what the caller keeps of them), the CRC-32 of every chunk before the first IDAT, consecutive IDATs, a
+    chunk after them.  -> (on_ihdr's result, (data offset, length) of every IDAT chunk, [(type, data)] of the chunks
+    before the first IDAT whose type is in `keep`, in file order)."""
     mv = memoryview(data)
     n = len(data)
     if n < 8 or data[:8] != PNG_SIGNATURE:
@@ -84,6 +117,7 @@ def parse_png(data: bytes) -> PngInfo:
     pos = 8
     ihdr = None
     idat: List[Tuple[int, int]] = []             # (file offset, length) of every IDAT chunk's data
+    kept = []
     while True:
         if pos + 8 > n:
             raise ValueError("truncated PNG (chunk header)")
@@ -104,15 +138,7 @@ def parse_png(data: bytes) -> PngInfo:
             W, H, depth, color, comp, filt, interlace = struct.unpack_from(">IIBBBBB", data, body)
             if W == 0 or H == 0 or W > 0x7FFFFFFF or H > 0x7FFFFFFF:
                 raise ValueError("bad image size")
-            if depth != 8 or color not in CHANNELS:
-                raise ValueError(f"unsupported PNG: bit depth {depth}, colour type {color}")
-            if comp != 0 or filt != 0:
-                raise ValueError("unknown compression or filter method")
-            if interlace != 0:
-                raise ValueError("unsupported PNG: interlaced")
-            if W * CHANNELS[color] > PNG_MAX_ROW_BYTES:
-                raise ValueError(f"unsupported PNG: rows of {W * CHANNELS[color]} bytes (at most {PNG_MAX_ROW_BYTES})")
-            ihdr = (W, H, CHANNELS[color])
+            ihdr = on_ihdr(W, H, depth, color, comp, filt, interlace)
         elif ctype == b"IDAT":
             if idat and idat[-1][0] + idat[-1][1] + 4 != pos:
                 raise ValueError("IDAT chunks are not consecutive")
@@ -121,14 +147,121 @@ def parse_png(data: bytes) -> PngInfo:
             break                                 # the image data ends at the first chunk after the IDATs
         elif ctype == b"IEND":
             raise ValueError("no IDAT chunk")
+        elif ctype in keep:
+            kept.append((ctype, bytes(mv[body: body + length])))
         pos = body + length + 4
-    W, H, C = ihdr
-    raw_len = H * (1 + W * C)
-    stream = _IdatStream(data, idat)
-    segs, inflated, trailer = _stored_segments(stream, raw_len)
-    info = PngInfo(W, H, C, segs, inflated, [(off - 8, ln) for off, ln in idat], trailer)
-    _check_filters(info, data)
+    return ihdr, idat, kept
+
+
+# --------------------------------------------------------------------------------------
+# every other PNG PIL opens: palette, 1/2/4/16-bit, Adam7 (csrc/usdu_png_decode.cu, general entry)
+# --------------------------------------------------------------------------------------
+GENERAL_CHANNELS = {0: 1, 2: 3, 3: 1, 4: 2, 6: 4}             # colour type -> samples per pixel
+GENERAL_DEPTHS = {0: (1, 2, 4, 8, 16), 2: (8, 16), 3: (1, 2, 4, 8), 4: (8, 16), 6: (8, 16)}
+ADAM7 = ((0, 0, 8, 8), (4, 0, 8, 8), (0, 4, 4, 8), (2, 0, 4, 4), (0, 2, 2, 4), (1, 0, 2, 2), (0, 1, 1, 2))
+
+
+class PngGeneral:
+    """A validated PNG of any colour type and bit depth, interlaced or not.  `inflated` is its filtered stream R: per
+    pass (one, or Adam7's seven back to back; a pass with no columns or rows has no bytes), per row a filter byte and
+    row_bytes(pass width) bytes.  `palette`: 768 bytes (PLTE's entries, then zeros) for colour type 3, else None."""
+    __slots__ = ("W", "H", "color", "depth", "interlace", "palette", "inflated")
+
+    def __init__(self, W, H, color, depth, interlace, palette=None, inflated=b""):
+        self.W, self.H, self.color, self.depth, self.interlace = W, H, color, depth, interlace
+        self.palette, self.inflated = palette, inflated
+
+    @property
+    def C(self) -> int:
+        return GENERAL_CHANNELS[self.color]
+
+    @property
+    def bpp(self) -> int:
+        """Bytes of a PNG filter unit: max(1, depth * C / 8)."""
+        return max(1, self.depth * self.C // 8)
+
+    def row_bytes(self, w: int) -> int:
+        return (w * self.depth * self.C + 7) // 8
+
+    def passes(self) -> List[Tuple[int, int, int, int, int, int, int]]:
+        """-> (x0, y0, dx, dy, pass width, pass height, offset in R) of every non-empty pass."""
+        out, at = [], 0
+        for x0, y0, dx, dy in (ADAM7 if self.interlace else ((0, 0, 1, 1),)):
+            pw, ph = max(0, (self.W - x0 + dx - 1) // dx), max(0, (self.H - y0 + dy - 1) // dy)
+            if pw and ph:
+                out.append((x0, y0, dx, dy, pw, ph, at))
+                at += ph * (1 + self.row_bytes(pw))
+        return out
+
+    @property
+    def raw_len(self) -> int:
+        return sum(ph * (1 + self.row_bytes(pw)) for _, _, _, _, pw, ph, _ in self.passes())
+
+
+def _ihdr_general(W, H, depth, color, comp, filt, interlace):
+    # PIL reads no compression method and takes any non-zero interlace byte as Adam7
+    if depth not in GENERAL_DEPTHS.get(color, ()):
+        raise ValueError(f"unsupported PNG: bit depth {depth}, colour type {color}")
+    if filt != 0:
+        raise ValueError("unknown filter method")
+    n = (W * depth * GENERAL_CHANNELS[color] + 7) // 8
+    if n > PNG_MAX_ROW_BYTES:
+        raise ValueError(f"unsupported PNG: rows of {n} bytes (at most {PNG_MAX_ROW_BYTES})")
+    return W, H, depth, color, int(interlace != 0)
+
+
+def parse_png_general(data: bytes) -> PngGeneral:
+    """Validate `data` as PIL's open().convert("RGB") reads any PNG and return it with its inflated filtered stream:
+    parse_png's chunk walk and CRC rule; every (colour type, depth) the PNG spec allows; PLTE (at most 256 entries, any
+    length) and tRNS (grey needs 2 bytes, RGB 6) as PIL reads them; the zlib stream inflated to its end, its Adler-32
+    included; every filter byte <= 4; filtered rows of at most PNG_MAX_ROW_BYTES.  ValueError with the reason
+    otherwise.  As with parse_png, a stream that ends before the image does, or a bad Adler-32 after a later IDAT
+    chunk, is refused although PIL, which stops reading once the last row is decoded, may take some such files."""
+    (W, H, depth, color, interlace), idat, kept = _walk_chunks(data, _ihdr_general, (b"PLTE", b"tRNS"))
+    palette = None
+    for ctype, body in kept:
+        if ctype == b"PLTE" and color == 3:
+            if len(body) // 3 > 256:
+                raise ValueError("invalid palette size")
+            palette = body[:len(body) // 3 * 3]
+        elif ctype == b"tRNS" and len(body) < {0: 2, 2: 6}.get(color, 0):
+            raise ValueError("tRNS chunk too short")
+    if color == 3:
+        palette = (palette or b"").ljust(768, b"\0")
+    info = PngGeneral(W, H, color, depth, interlace, palette)
+    st = _IdatStream(data, idat)
+    hdr = st.read(0, 2)
+    cmf, flg = hdr[0], hdr[1]
+    if (cmf & 0x0F) != 8 or (cmf >> 4) > 7 or (cmf * 256 + flg) % 31 != 0 or (flg & 0x20):
+        raise ValueError("bad zlib header")
+    d = zlib.decompressobj()
+    try:
+        out = d.decompress(st.joined(), info.raw_len)
+        while not d.eof:                          # the rest up to the stream's end, its Adler-32 included
+            if not d.decompress(d.unconsumed_tail, 1 << 20) and not d.unconsumed_tail:
+                break
+    except zlib.error as e:
+        raise ValueError(f"broken deflate stream: {e}") from None
+    if not d.eof:
+        raise ValueError("image data is truncated")
+    if len(out) < info.raw_len:
+        # as parse_png: PIL takes some streams that end early on a row's end, depending on how IDAT is cut; not these
+        raise ValueError("image data is truncated")
+    info.inflated = out
+    R = np.frombuffer(info.inflated, np.uint8)
+    for _, _, _, _, pw, ph, at in info.passes():
+        if int(R[at: at + ph * (1 + info.row_bytes(pw)): 1 + info.row_bytes(pw)].max()) > 4:
+            raise ValueError("unrecognized data stream contents (filter type > 4)")
     return info
+
+
+def parse_png_any(data: bytes):
+    """parse_png, or parse_png_general for a file parse_png refuses only for its depth, colour type or interlace.
+    -> PngInfo (the 8-bit fast path) or PngGeneral."""
+    try:
+        return parse_png(data)
+    except UnsupportedPng:
+        return parse_png_general(data)
 
 
 class _IdatStream:
@@ -429,7 +562,7 @@ def parse_tiles_from_form(data) -> List[dict]:
             raise ValueError(f"Missing tile data for index {i}")
         raw = field.file.read()
         try:
-            info = parse_png(raw)
+            info = parse_png_any(raw)
         except Exception as e:
             raise ValueError(f"Invalid image data for tile {i}: {e}")
         try:
@@ -534,7 +667,7 @@ def make_handlers(store: JobStore):
                 int(data.get("image_idx"))
                 img = data["full_image"].file.read()
                 try:
-                    parse_png(img)
+                    parse_png_any(img)
                 except ValueError as e:
                     return _error(e, 500)
             elif not is_last:
@@ -666,8 +799,56 @@ class PngDecoder:
         self._events = []
         self._keep_alive = []
 
-    def decode(self, items: Sequence[Tuple[PngInfo, bytes, int]], dst):
-        """items: (info, PNG bytes, byte offset of the frame's [H, W, 3] u8 output in the device tensor `dst`)."""
+    def decode(self, items: Sequence[Tuple[object, bytes, int]], dst) -> int:
+        """items: (PngInfo or PngGeneral, PNG bytes, byte offset of the frame's [H, W, 3] u8 output in the device tensor
+        `dst`).  The 8-bit frames go to usdu_png_decode_u8, the others to usdu_png_decode_general_u8, on the side
+        stream.  -> launches made."""
+        general = [it for it in items if isinstance(it[0], PngGeneral)]
+        fast = [it for it in items if not isinstance(it[0], PngGeneral)]
+        self._decode_fast(fast, dst)
+        self.decode_general([(info, off) for info, _, off in general], dst)
+        return int(bool(fast)) + int(bool(general))
+
+    def decode_general(self, items: Sequence[Tuple[PngGeneral, int]], dst):
+        """items: (PngGeneral, byte offset of the frame's output in `dst`): each frame's R and palette uploaded through
+        pinned memory, one CTA per (frame, pass) in one usdu_png_decode_general_u8 launch."""
+        import torch
+        from . import _native as nat
+        if not items:
+            return
+        blobs, descs, pos, max_row = [], [], 0, 1
+        for info, off in items:
+            pal = pos
+            if info.palette is not None:
+                blobs.append(info.palette)
+                pos += len(info.palette)
+            for x0, y0, dx, dy, pw, ph, at in info.passes():
+                descs.append([pos + at, pw, ph, x0, y0, dx, dy, info.W, info.color, info.depth, off, pal, 0, 0, 0, 0])
+                max_row = max(max_row, info.row_bytes(pw))
+            blobs.append(info.inflated)
+            pos += len(info.inflated)
+        tabs = np.asarray(descs, np.int64).reshape(-1)
+        t0 = (pos + 15) // 16 * 16
+        host = torch.empty(t0 + tabs.nbytes, dtype=torch.uint8, pin_memory=True)
+        h = host.numpy()
+        o = 0
+        for blob in blobs:
+            h[o: o + len(blob)] = np.frombuffer(blob, np.uint8)
+            o += len(blob)
+        h[t0:] = tabs.view(np.uint8)
+        with torch.cuda.device(self.device), torch.cuda.stream(self.side):
+            dev = torch.empty(host.numel(), dtype=torch.uint8, device=self.device)
+            e_up, e0, e1 = (torch.cuda.Event(enable_timing=True) for _ in range(3))
+            e_up.record(self.side)
+            dev.copy_(host, non_blocking=True)
+            e0.record(self.side)
+            nat.png_decode_general_u8(dev.data_ptr(), dev.data_ptr() + t0, len(descs), max_row, dst.data_ptr(),
+                                      self.side.cuda_stream)
+            e1.record(self.side)
+        self._events.append((e_up, e0, e1))
+        self._keep_alive.append((host, dev, dst))
+
+    def _decode_fast(self, items: Sequence[Tuple[PngInfo, bytes, int]], dst):
         import torch
         from . import _native as nat
         if not items:
@@ -785,7 +966,8 @@ class HttpStaticMaster:
 
     # -- decode as results arrive ---------------------------------------------------------
     def _decode(self, entries: List[Tuple[int, dict]]):
-        """Upload the PNG bytes of `entries` through pinned memory and decode them on the side stream."""
+        """Upload the PNG bytes (or, for a PngGeneral, the filtered stream) of `entries` through pinned memory and
+        decode them on the side stream."""
         items = []
         for g, e in entries:
             b = e.get("batch_idx", g // self.T)
@@ -801,8 +983,7 @@ class HttpStaticMaster:
         if not items:
             return
         self.stats["tiles_received"] += len(items)
-        self.decoder.decode(items, self.payload)
-        self.stats["decode_launches"] += 1
+        self.stats["decode_launches"] += self.decoder.decode(items, self.payload)
 
     # -- the job --------------------------------------------------------------------------
     def run(self):

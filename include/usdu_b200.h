@@ -35,7 +35,7 @@ extern "C" {
 #pragma GCC visibility push(default) /* the library itself is built with -fvisibility=hidden */
 #endif
 
-#define USDU_ABI_VERSION 17
+#define USDU_ABI_VERSION 18
 
 typedef enum usdu_status {
     USDU_OK = 0,
@@ -329,6 +329,23 @@ int usdu_png_base64_u8(const uint8_t* src_dev, int B, int H, int W, int C, uint8
 int usdu_png_decode_u8(const uint8_t* src_dev, const int64_t* segs_dev, int64_t n_segs, const int64_t* descs_dev,
                        int n, int max_row_bytes, uint8_t* dst_dev, void* stream);
 int usdu_png_decode_warps(int max_row_bytes);
+
+/* The same decode for every other PNG PIL's open().convert("RGB") opens: colour type 0 at 1/2/4/8/16 bits, 2 at 8/16,
+ * 3 (palette) at 1/2/4/8, 4 and 6 at 8/16, interlaced (Adam7) or not.  The host inflates each file's zlib stream
+ * (http_master.parse_png_general) and uploads the filtered stream R whole; a frame is one pass, or Adam7's seven
+ * (the empty ones left out), each decoded by one CTA of the launch.
+ * descs_dev: n pass descriptors of USDU_PNG_GENERAL_DESC_WORDS int64: offset in src_dev of the pass's R (per row a
+ *   filter byte 0..4, then ceil(w * depth * C / 8) bytes), pass width w >= 1 and height h >= 1, x0, y0, dx, dy (pixel
+ *   (i, j) of the pass is pixel (y0 + i*dy, x0 + j*dx) of the frame; 0, 0, 1, 1 without interlace), the frame's width,
+ *   colour type, bit depth, byte offset of the frame's [H, W, 3] u8 output in dst_dev, offset in src_dev of a
+ *   768-byte RGB palette (colour type 3: the PLTE's entries, zeros after them), then 0s.
+ * The rows are un-filtered on PNG filter units of max(1, depth * C / 8) bytes and converted as PIL 12's
+ * convert("RGB"): 1/2/4-bit grey times 255/85/17, 16-bit grey min(v, 255), other 16-bit samples their high byte,
+ * palette indices through the palette (tRNS ignored), grey replicated, alpha dropped.  max_row_bytes >= every pass's
+ * filtered row bytes and <= USDU_PNG_MAX_ROW_BYTES; the ring depth is usdu_png_decode_warps(max_row_bytes). */
+#define USDU_PNG_GENERAL_DESC_WORDS 16
+int usdu_png_decode_general_u8(const uint8_t* src_dev, const int64_t* descs_dev, int n, int max_row_bytes,
+                               uint8_t* dst_dev, void* stream);
 
 /* HTTP tile worker transport (upscale/worker_comms.py:30-34): each u8 RGB frame [H, W, 3] as the PNG Pillow writes with
  * compress_level=0, byte for byte.  At level 0 Pillow's file is a framing that depends on the shape alone, filled with
