@@ -7,6 +7,6 @@ ComfyUI loads this directory as a custom node package and reads NODE_CLASS_MAPPI
 from .nodes import NODE_CLASS_MAPPINGS, NODE_DISPLAY_NAME_MAPPINGS
 from .http_master import install_in_comfyui as _install_routes
 
-_install_routes()      # inside ComfyUI: serve the static-mode master's routes (http_master.py)
+_install_routes()      # inside ComfyUI: serve the masters' routes (http_master.py, http_collector.py, orchestrator.py)
 
 __all__ = ["NODE_CLASS_MAPPINGS", "NODE_DISPLAY_NAME_MAPPINGS"]
