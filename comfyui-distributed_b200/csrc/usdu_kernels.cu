@@ -916,7 +916,8 @@ int usdu_tile_crop_resize(const uint8_t* canvas_dev, int B, int H, int W, int64_
 int usdu_tile_crop_resize_f32(const float* image_dev, int B, int H, int W, const int32_t* tabs_dev, const int32_t* items_dev,
                               int n_items, int patch_w, int patch_h, float* out_dev, int flags, void* stream) {
     USDU_REQUIRE(image_dev && tabs_dev && items_dev && out_dev, "usdu_tile_crop_resize_f32: null pointer");
-    USDU_REQUIRE(B > 0 && H > 0 && W > 0 && n_items >= 0 && B <= 65535, "usdu_tile_crop_resize_f32: bad shape");
+    USDU_REQUIRE(B > 0 && H > 0 && W > 0 && n_items >= 0, "usdu_tile_crop_resize_f32: bad shape");
+    USDU_REQUIRE(B <= 65535, "usdu_tile_crop_resize_f32: batch %d exceeds grid.y limit", B);
     USDU_REQUIRE(flags & USDU_FLAG_MMA, "usdu_tile_crop_resize_f32: tensor-core job records only (USDU_FLAG_MMA)");
     if (n_items == 0) return USDU_OK;
     return mma::launch_crop(image_dev, 1, B, H, W, (int64_t)W * 3, tabs_dev, items_dev, n_items, patch_w, patch_h, out_dev,

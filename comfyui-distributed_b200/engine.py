@@ -32,6 +32,18 @@ def _stream_ptr() -> int:
     return torch.cuda.current_stream().cuda_stream
 
 
+# Every frame of a batch is one grid.y index of the crop and blend launches, whose limit is 65,535.  A larger batch is
+# refused before any device work.  It is not run in chunks: a sampler sees the whole batch per tile, so chunking would
+# change the noise it draws.
+MAX_BATCH = 65535
+
+
+def check_batch(B: int):
+    if B > MAX_BATCH:
+        raise ValueError(f"Batch size {B} exceeds {MAX_BATCH} frames, the most one tile launch takes. "
+                         "Please split the batch.")
+
+
 class KernelProfile:
     """Optional per-launch CUDA-event timing on the launching stream (bench.py's roofline).
     Usage: prof = KernelProfile(); engine.PROFILE = prof; ...; prof.summary()."""
@@ -694,6 +706,7 @@ def upscale_single(image: torch.Tensor, denoiser: Denoiser, tile_width: int, til
                    use_graph: Optional[bool] = None, _skip: Sequence[str] = ()) -> torch.Tensor:
     """One-GPU job on a CUDA image [B,H,W,3] fp32 -> fp32 (values k/255), exact
     progressive semantics of process_single_gpu."""
+    check_batch(int(image.shape[0]))
     _require_cuda(image, "image")
     B, H, W, _ = image.shape
     plan = get_plan(W, H, tile_width, tile_height, padding, mask_blur, force_uniform_tiles)
@@ -1006,6 +1019,7 @@ def upscale_host(host_image: torch.Tensor, denoiser: Denoiser, tile_width: int, 
     of the two PCIe streams; the extra small launches hide under the copies)."""
     if host_image.is_cuda:
         raise ValueError("upscale_host takes a host tensor; use upscale_single for device tensors")
+    check_batch(int(host_image.shape[0]))
     device = device or torch.device("cuda", torch.cuda.current_device())
     x = reference_f32(host_image).contiguous()
     B, H, W, _ = x.shape

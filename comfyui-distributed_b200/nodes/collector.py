@@ -28,6 +28,7 @@ from .. import http_collector, http_worker
 from ..casts import reference_f32
 
 PNG_TEXT_BUDGET = 64 << 20    # pinned host bytes for one group of frames' base64 text (at least one frame)
+PNG_MAX_GROUP = 65535         # frames of one usdu_png_base64_u8 launch (one per grid.y index)
 
 
 def _native_pack(images: torch.Tensor) -> torch.Tensor:
@@ -57,8 +58,8 @@ _text_pool = None
 
 def _native_png_b64(q: torch.Tensor):
     """u8 CUDA frames [B,H,W,C] -> each frame's base64 PNG text in batch order (usdu_png_base64_u8).  Frames are encoded
-    in groups whose text fits PNG_TEXT_BUDGET; a group's text is copied to pinned host memory once.  Each item is a
-    memoryview into that buffer, valid until the next item is requested."""
+    in groups of at most PNG_MAX_GROUP frames whose text fits PNG_TEXT_BUDGET; a group's text is copied to pinned host
+    memory once.  Each item is a memoryview into that buffer, valid until the next item is requested."""
     global _text_pool
     from .. import _native as nat
     from ..engine import _PinnedPool
@@ -66,7 +67,7 @@ def _native_png_b64(q: torch.Tensor):
     if B == 0:
         return
     _, text_len, staging_len = nat.png_sizes(H, W, C)
-    group = max(1, min(B, PNG_TEXT_BUDGET // text_len))
+    group = max(1, min(B, PNG_TEXT_BUDGET // text_len, PNG_MAX_GROUP))
     q = q.contiguous()
     if _text_pool is None:
         _text_pool = _PinnedPool(keep=1, shapes=2)

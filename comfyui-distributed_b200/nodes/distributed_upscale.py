@@ -28,7 +28,7 @@ from .. import dist as usdu_dist
 from .. import http_master
 from ..casts import reference_f32
 from ..denoise import ComfySampler
-from ..engine import WorkerJob, upscale_host, upscale_single
+from ..engine import WorkerJob, check_batch, upscale_host, upscale_single
 from ..http_worker import HttpStaticWorker
 
 try:  # ComfyUI supplies these lists; outside ComfyUI keep the signature importable
@@ -113,6 +113,7 @@ class UltimateSDUpscaleDistributed:
                 f"Batch size {batch_size} is not of the form 4n+1. "
                 "This node requires batch sizes of 1 or 4n+1 (1, 5, 9, 13, ...). "
                 "Please adjust the batch size.")
+        check_batch(batch_size)              # both roles: one frame per grid.y index of the tile launches
         if multi_job_id:
             json.loads(enabled_worker_ids)   # raw parse like :175/:227 -> JSONDecodeError propagates
 
