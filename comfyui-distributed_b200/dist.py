@@ -718,6 +718,16 @@ def _payload_buffer(nbytes: int, device) -> torch.Tensor:
     return _PAYLOADS.get_or_build(key, lambda: torch.zeros(int(nbytes), dtype=torch.uint8, device=device))
 
 
+def release_caches():
+    """Drop the cached peer buffers, static and exact jobs and send buffers (engine.release_device_caches) -- unless a
+    process group of more than one rank is initialised: those entries are created collectively, and one rank dropping
+    them alone would desynchronise the ranks."""
+    if dist_info()[1] > 1:
+        return
+    for cache in (StaticJob._cache, ExactJob._cache, PeerPayload._cache, _PAYLOADS):
+        cache.clear()
+
+
 class ExactJob:
     """Per-geometry state of `semantics="exact"` jobs: for every dependency wave the round-robin shares, the payload
     layout, the send buffer and the gathered buffer (all sizes follow from the plan: no size exchange, no host sync,

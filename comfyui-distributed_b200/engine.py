@@ -7,7 +7,9 @@ upscale/modes/static.py (per-participant canvases, sorted final blend :521-553).
 """
 from __future__ import annotations
 
+import contextlib
 import os
+import threading
 from typing import Callable, Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
@@ -1042,3 +1044,55 @@ def upscale_host(host_image: torch.Tensor, denoiser: Denoiser, tile_width: int, 
         stats["algo_bytes"] = stats.get("algo_bytes", 0) + hp.canvas.algo_bytes
         stats["tiles"], stats["bands"] = len(plan.tiles), len(hp.bands)
     return out
+
+
+# --------------------------------------------------------------------------------------
+# releasing the caches (POST /distributed/clear_memory, worker_routes.py)
+# --------------------------------------------------------------------------------------
+_jobs_lock = threading.Lock()       # guards the two below; every release of the caches happens under it
+_jobs_running = 0
+_release_pending = False
+
+
+@contextlib.contextmanager
+def job_scope():
+    """The extent of one node run (UltimateSDUpscaleDistributed, DistributedCollector).  A release asked for while jobs
+    run is done by the last of them to leave, so no cached canvas or graph is dropped while a job may still use it."""
+    global _jobs_running
+    with _jobs_lock:
+        _jobs_running += 1
+    try:
+        yield
+    finally:
+        with _jobs_lock:
+            _jobs_running -= 1
+            if _jobs_running == 0 and _release_pending:
+                _release_locked()
+
+
+def release_device_caches():
+    """Drop this package's device caches: the DevicePlan, GraphedWaves and HostPipeline entries, the pinned result and
+    staging pools, the collector's text pool and dist's jobs and buffers (dist.release_caches).  A pool drops only its
+    own reference: a result the caller still holds stays alive.  While a job runs the release is left to the last job
+    to finish."""
+    global _release_pending
+    with _jobs_lock:
+        if _jobs_running:
+            _release_pending = True
+        else:
+            _release_locked()
+
+
+def _release_locked():
+    global _release_pending
+    from . import dist
+    from .nodes import collector
+    _release_pending = False
+    devices = {dp.device for dp in DevicePlan._cache.values()} | \
+        {gw.canvas.dp.device for gw in GraphedWaves._cache.values()} | {hp.dp.device for hp in HostPipeline._cache.values()}
+    for dev in devices:
+        torch.cuda.synchronize(dev)             # nothing still in flight reads what is dropped
+    for cache in (GraphedWaves._cache, HostPipeline._cache, DevicePlan._cache, PINNED_RESULTS.bufs, PINNED_STAGING.bufs):
+        cache.clear()
+    collector._text_pool = None
+    dist.release_caches()

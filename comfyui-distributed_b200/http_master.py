@@ -744,8 +744,8 @@ def register(routes, store: JobStore = STORE, loop=None) -> set:
 
 
 def install_in_comfyui():
-    """Register the routes of this module, of http_collector and of the orchestrator on server.PromptServer.instance
-    when imported inside ComfyUI; a no-op elsewhere."""
+    """Register the routes of this module, of http_collector, of the orchestrator and of worker_routes on
+    server.PromptServer.instance when imported inside ComfyUI; a no-op elsewhere."""
     try:
         import server
         inst = server.PromptServer.instance
@@ -755,9 +755,10 @@ def install_in_comfyui():
         return
     if not _served:
         register(inst.routes, STORE, getattr(inst, "loop", None))
-    from . import http_collector, orchestrator
+    from . import http_collector, orchestrator, worker_routes
     http_collector.install(inst.routes, getattr(inst, "loop", None))
     orchestrator.install(inst)
+    worker_routes.install(inst)
 
 
 def serving() -> bool:

@@ -26,6 +26,7 @@ import torch
 from .. import dist as usdu_dist
 from .. import http_collector, http_worker
 from ..casts import reference_f32
+from ..engine import job_scope
 
 PNG_TEXT_BUDGET = 64 << 20    # pinned host bytes for one group of frames' base64 text (at least one frame)
 PNG_MAX_GROUP = 65535         # frames of one usdu_png_base64_u8 launch (one per grid.y index)
@@ -179,6 +180,7 @@ class DistributedCollectorNode:
     FUNCTION = "run"
     CATEGORY = "image"
 
+    @job_scope()
     def run(self, images, load_balance=False, audio=None, multi_job_id="", is_worker=False, master_url="",
             enabled_worker_ids="[]", worker_batch_size=1, worker_id="", pass_through=False, delegate_only=False):
         empty_audio = {"waveform": torch.zeros(1, 2, 1), "sample_rate": 44100}

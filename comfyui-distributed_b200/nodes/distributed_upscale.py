@@ -28,7 +28,7 @@ from .. import dist as usdu_dist
 from .. import http_master
 from ..casts import reference_f32
 from ..denoise import ComfySampler
-from ..engine import WorkerJob, check_batch, upscale_host, upscale_single
+from ..engine import WorkerJob, check_batch, job_scope, upscale_host, upscale_single
 from ..http_worker import HttpStaticWorker
 
 try:  # ComfyUI supplies these lists; outside ComfyUI keep the signature importable
@@ -96,6 +96,7 @@ class UltimateSDUpscaleDistributed:
         return ComfySampler(model, positive, negative, vae, seed, steps, cfg, sampler_name, scheduler, denoise,
                             tiled_decode=tiled_decode, image_size=image_size, cond_cropper=make_cond_cropper())
 
+    @job_scope()
     def run(self, upscaled_image, model, positive, negative, vae, seed, steps, cfg, sampler_name, scheduler,
             denoise, tile_width, tile_height, padding, mask_blur, force_uniform_tiles, tiled_decode,
             multi_job_id="", is_worker=False, master_url="", enabled_worker_ids="[]", worker_id="",

@@ -13,8 +13,9 @@ roles of http_master.py and http_collector.py.  No pixel work happens here.
 HTTP goes through one aiohttp session per request that reads no proxy from the environment (as http_worker.py).
 
 Differences from the reference (INTEGRATION.md, "The orchestrator"):
-* `websocket_orchestration: true` (the reference's default) needs `/distributed/worker_ws` on the workers; this package
-  probes and dispatches over HTTP instead and warns once;
+* `websocket_orchestration: true` (the reference's default) probes and dispatches over `/distributed/worker_ws`; workers
+  running this package serve it (worker_routes.py), but this orchestrator still probes and dispatches over HTTP and
+  warns once;
 * the config file is only read: its editing routes belong to the reference's web UI.
 """
 from __future__ import annotations
@@ -572,6 +573,39 @@ class PromptValidationError(RuntimeError):
         super().__init__(f"Invalid prompt: {merged}")
 
 
+async def queue_prompt(server, prompt: dict, workflow_meta, client_id, validate=None) -> dict:
+    """Validate and queue a prompt on this ComfyUI, as its POST /prompt does -> {prompt_id, number, node_errors}.
+    `server`: the PromptServer (trigger_on_prompt, number, prompt_queue); `validate`: execution.validate_prompt when
+    None.  A refused prompt raises PromptValidationError."""
+    if validate is None:
+        import execution
+        validate = execution.validate_prompt
+    prompt = server.trigger_on_prompt({"prompt": prompt})["prompt"]
+    prompt_id = str(uuid.uuid4())
+    valid = await validate(prompt_id, prompt, None)
+    if not valid[0]:
+        raise PromptValidationError(valid[1] if len(valid) > 1 else "Prompt outputs failed validation",
+                                    valid[3] if len(valid) > 3 else {})
+    extra = {"create_time": int(time.time() * 1000)}
+    if workflow_meta:
+        extra["extra_pnginfo"] = {"workflow": workflow_meta}
+    if client_id:
+        extra["client_id"] = client_id
+    sensitive = {}
+    try:
+        import execution
+        keys = getattr(execution, "SENSITIVE_EXTRA_DATA_KEYS", [])
+    except ImportError:
+        keys = []
+    for key in keys:
+        if key in extra:
+            sensitive[key] = extra.pop(key)
+    number = getattr(server, "number", 0)
+    server.number = number + 1
+    server.prompt_queue.put((number, prompt_id, prompt, extra, valid[2], sensitive))
+    return {"prompt_id": prompt_id, "number": number, "node_errors": {}}
+
+
 # --------------------------------------------------------------------------------------
 # the orchestration (api/queue_orchestration.py, api/orchestration/dispatch.py)
 # --------------------------------------------------------------------------------------
@@ -583,8 +617,7 @@ def _warn_websocket_once():
     if not _ws_warned:
         _ws_warned = True
         warnings.warn("comfyui-distributed_b200: websocket_orchestration is set, but this package dispatches worker "
-                      "prompts over HTTP (POST /prompt); /distributed/worker_ws is not served", RuntimeWarning,
-                      stacklevel=3)
+                      "prompts over HTTP (POST /prompt)", RuntimeWarning, stacklevel=3)
 
 
 class Orchestrator:
@@ -735,37 +768,6 @@ class Orchestrator:
             return chosen
         return min(statuses, key=lambda s: s[1])[0]
 
-    async def queue_master(self, prompt: dict, workflow_meta, client_id):
-        """Validate and queue a prompt on this ComfyUI, as its POST /prompt does -> {prompt_id, number, node_errors}."""
-        validate = self._validate
-        if validate is None:
-            import execution
-            validate = execution.validate_prompt
-        prompt = self.server.trigger_on_prompt({"prompt": prompt})["prompt"]
-        prompt_id = str(uuid.uuid4())
-        valid = await validate(prompt_id, prompt, None)
-        if not valid[0]:
-            raise PromptValidationError(valid[1] if len(valid) > 1 else "Prompt outputs failed validation",
-                                        valid[3] if len(valid) > 3 else {})
-        extra = {"create_time": int(time.time() * 1000)}
-        if workflow_meta:
-            extra["extra_pnginfo"] = {"workflow": workflow_meta}
-        if client_id:
-            extra["client_id"] = client_id
-        sensitive = {}
-        try:
-            import execution
-            keys = getattr(execution, "SENSITIVE_EXTRA_DATA_KEYS", [])
-        except ImportError:
-            keys = []
-        for key in keys:
-            if key in extra:
-                sensitive[key] = extra.pop(key)
-        number = getattr(self.server, "number", 0)
-        self.server.number = number + 1
-        self.server.prompt_queue.put((number, prompt_id, prompt, extra, valid[2], sensitive))
-        return {"prompt_id": prompt_id, "number": number, "node_errors": {}}
-
     def session(self):
         """The HTTP client of one request (aiohttp reads no proxy from the environment unless told to)."""
         import aiohttp
@@ -811,7 +813,7 @@ class Orchestrator:
         enabled_ids = [w["id"] for w in active]
         jobs = job_id_map(index, self.job_prefix())
         if not jobs:
-            queued = await self.queue_master(prompt, workflow_meta, client_id)
+            queued = await queue_prompt(self.server, prompt, workflow_meta, client_id, self._validate)
             return queued["prompt_id"], queued["number"], 0, queued.get("node_errors", {})
         for job in jobs.values():
             await self.store.prepare(job)
@@ -845,7 +847,7 @@ class Orchestrator:
         prepared = await asyncio.gather(*[prepare(w) for w in active]) if active else []
         if prepared:
             await asyncio.gather(*[self.dispatch(session, w, wp, workflow_meta) for w, wp in prepared])
-        queued = await self.queue_master(master_prompt, workflow_meta, client_id)
+        queued = await queue_prompt(self.server, master_prompt, workflow_meta, client_id, self._validate)
         return queued["prompt_id"], queued["number"], len(prepared), queued.get("node_errors", {})
 
 
