@@ -16,7 +16,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libusdu_b200.so")
 
 # constants mirrored from include/usdu_b200.h (checked against the header in tests)
-ABI_VERSION = 18
+ABI_VERSION = 19
 ERR_INVALID = -1
 CANVAS_SLACK = 16
 PLAN_INFO_WORDS = 16
@@ -95,6 +95,9 @@ _SIGNATURES = {
     "usdu_png_decode_u8": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "usdu_png_decode_warps": (c_int, [c_int]),
     "usdu_png_decode_general_u8": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    "usdu_jpeg_parse": (c_int, [c_void_p, c_int64, POINTER(c_int64), POINTER(c_int32)]),
+    "usdu_jpeg_decode_coefs": (c_int, [c_void_p, c_int64, c_void_p, c_int64]),
+    "usdu_jpeg_decode_u8": (c_int, [c_void_p, c_void_p, c_int, c_int64, c_void_p, c_void_p]),
     "usdu_png_encode_u8": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int64, c_void_p, c_int, c_void_p,
                                    c_int, POINTER(c_int64), c_void_p, c_void_p, c_void_p]),
     "usdu_gather_unpack_f32": (c_int, [c_void_p, c_int, c_int64, c_void_p, c_void_p]),
@@ -494,6 +497,41 @@ def png_decode_general_u8(src_ptr, descs_ptr, n, max_row_bytes, dst_ptr, stream)
     (usdu_png_decode_general_u8)."""
     _check(lib().usdu_png_decode_general_u8(src_ptr, descs_ptr, n, max_row_bytes, dst_ptr, stream),
            "usdu_png_decode_general_u8")
+
+
+# baseline JPEG (include/usdu_b200.h): the host parse and Huffman decode, then the device stages
+JPEG_INFO_WORDS = 16
+(JI_W, JI_H, JI_COMPONENTS, JI_H0, JI_V0, JI_COLOUR, JI_RESTART, JI_MCUX, JI_MCUY, JI_BLOCKS, JI_SCAN) = range(11)
+JPEG_GREY, JPEG_YCC, JPEG_RGB = 0, 1, 2
+JPEG_DESC_WORDS = 16
+JPEG_TILE_W = 128
+
+
+def jpeg_parse(data: bytes):
+    """-> (info int64 [JPEG_INFO_WORDS], quant int32 [3, 64]), or ValueError with the library's reason
+    (usdu_jpeg_parse)."""
+    info = np.zeros(JPEG_INFO_WORDS, np.int64)
+    quant = np.zeros((3, 64), np.int32)
+    st = lib().usdu_jpeg_parse(data, len(data), _i64p(info), quant.ctypes.data_as(POINTER(c_int32)))
+    if st == ERR_INVALID:
+        raise ValueError(lib().usdu_last_error().decode())
+    _check(st, "usdu_jpeg_parse")
+    return info, quant
+
+
+def jpeg_decode_coefs(data: bytes, coefs: np.ndarray):
+    """The Huffman decode of `data` into `coefs` (int16, 64 * info[JI_BLOCKS] words, any host memory, written in
+    place), or ValueError with the library's reason (usdu_jpeg_decode_coefs)."""
+    assert coefs.dtype == np.int16 and coefs.flags["C_CONTIGUOUS"]
+    st = lib().usdu_jpeg_decode_coefs(data, len(data), coefs.ctypes.data, coefs.size)
+    if st == ERR_INVALID:
+        raise ValueError(lib().usdu_last_error().decode())
+    _check(st, "usdu_jpeg_decode_coefs")
+
+
+def jpeg_decode_u8(src_ptr, descs_ptr, n, n_ctas, dst_ptr, stream):
+    """n frame descriptors (JPEG_DESC_WORDS int64, device) over src -> u8 RGB frames in dst (usdu_jpeg_decode_u8)."""
+    _check(lib().usdu_jpeg_decode_u8(src_ptr, descs_ptr, n, n_ctas, dst_ptr, stream), "usdu_jpeg_decode_u8")
 
 
 def png_encode_scratch_bytes(B: int, H: int, W: int) -> int:

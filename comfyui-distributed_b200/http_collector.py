@@ -14,6 +14,8 @@ model holds), or for what the device tables do not settle (compressed blocks, mo
 holds), the host path png_of_payload answers as the reference does (`b64decode(validate=True)`, then parse_png).  A
 palette, 1/2/4/16-bit or interlaced PNG, which parse_png refuses for its IHDR, is validated and inflated on the host by
 http_master.parse_png_general (the device path hands it the decoded bytes) and decoded with usdu_png_decode_general_u8.
+A baseline JPEG (base64 text starting "/9j/") always takes the host path, off the event loop: b64decode, then the
+library's marker parse and Huffman decode (http_master.parse_jpeg); usdu_jpeg_decode_u8 does the rest on the device.
 Both paths give every body the same answer.  The master decodes each drained batch of frames on a side stream (http_master.PngDecoder), from the
 device buffers or through a pinned upload, while it waits for more, and assembles the result with one
 usdu_gather_unpack_f32 launch that writes every worker frame, as k / 255, straight into the pinned host result in its
@@ -21,8 +23,9 @@ final order.
 
 Differences from the reference (INTEGRATION.md, "A master for HTTP workers"):
 * images PIL would open but this module refuses answer the reference's decode-failure response (500, "Failed to
-  decode PNG image payload: ..."): PNGs with filtered rows over PNG_MAX_ROW_BYTES (16,384 8-bit RGBA pixels) and other
-  formats PIL detects (JPEG, BMP, ...).  Neither worker sends any of them;
+  decode PNG image payload: ..."): PNGs with filtered rows over PNG_MAX_ROW_BYTES (16,384 8-bit RGBA pixels), JPEGs
+  outside the baseline subset http_master.parse_jpeg takes, and other formats PIL detects (BMP, GIF, ...).  Neither
+  worker sends any of them;
 * no busy-probe of missing workers (collector.py:374-411 reads the orchestrator's gpu_config.json), and the worker
   timeout is COMFYUI_HEARTBEAT_TIMEOUT (default 60 s), not the config file's setting;
 * delegate-only mode comes from the node's hidden input only, not from the config file;
@@ -44,8 +47,8 @@ from typing import Callable, Dict, List, Optional, Sequence, Tuple
 import numpy as np
 
 from . import _native as nat
-from .http_master import (CHANNELS, PNG_MAX_ROW_BYTES, PNG_SIGNATURE, PngInfo, UnsupportedPng, _IdatStream,
-                          heartbeat_interval, heartbeat_timeout, parse_png, parse_png_any, parse_png_general)
+from .http_master import (CHANNELS, PNG_MAX_ROW_BYTES, PNG_SIGNATURE, JpegInfo, PngInfo, UnsupportedPng, _IdatStream,
+                          heartbeat_interval, heartbeat_timeout, parse_image_any, parse_png, parse_png_general)
 
 JOB_INIT_GRACE_PERIOD = 10.0        # utils/constants.py:37: how long a POST waits for its job's queue
 GRACE_POLL = 0.05                   # job_routes.py:333
@@ -97,8 +100,8 @@ def payload_text(image: str) -> str:
 
 
 def png_of_payload(image: str) -> Tuple[bytes, PngInfo]:
-    """The image field -> (PNG bytes, their validation: PngInfo, or PngGeneral for a palette, 1/2/4/16-bit or
-    interlaced PNG), or ValueError with the reference's message: the host path."""
+    """The image field -> (image bytes, their validation: PngInfo, PngGeneral for a palette, 1/2/4/16-bit or
+    interlaced PNG, JpegInfo for a baseline JPEG), or ValueError with the reference's message: the host path."""
     text = payload_text(image)
     try:
         png = base64.b64decode(text, validate=True)
@@ -107,7 +110,7 @@ def png_of_payload(image: str) -> Tuple[bytes, PngInfo]:
     if not png:
         raise ValueError(EMPTY_PNG)
     try:
-        info = parse_png_any(png)
+        info = parse_image_any(png)
     except Exception as exc:
         raise ValueError(f"{PNG_FAILED}{exc}") from exc
     return png, info
@@ -245,7 +248,9 @@ def check_png_tables(tab: np.ndarray, m: int) -> PngInfo:
 # --------------------------------------------------------------------------------------
 # the device path of the image checks
 # --------------------------------------------------------------------------------------
-POOL_BYTES = 4 << 30        # device bytes of decoded PNGs held at once: 81 4K RGB frames are about 2 GB
+POOL_BYTES = 4 << 30        # bytes of decoded PNGs (device) and JPEG coefficients (host) held at once: 81 4K RGB
+                            # frames are about 2 GB
+JPEG_B64 = "/9j/"           # the base64 text of a body that starts with the JPEG SOI (FF D8 FF)
 WAIT_POLL = 0.0005          # s between polls of a CUDA event on the loop
 
 
@@ -268,6 +273,12 @@ class DevicePool:
 
     def give(self, nbytes: int):
         self.used -= nbytes
+
+    def hold(self, coefs: np.ndarray):
+        """Count a JPEG's host coefficient buffer, queued for the master's decode, until it is dropped: it stands in
+        for the decoded bytes a PNG keeps on the device, so PNGs that arrive while it waits see the bound sooner."""
+        self.used += coefs.nbytes
+        weakref.finalize(coefs, self.give, coefs.nbytes)
 
 
 class DevicePng:
@@ -316,7 +327,7 @@ class DeviceChecks:
         with torch.cuda.device(self.device):
             self.stream = torch.cuda.Stream(self.device)
         self.pool = pool if pool is not None else DevicePool()
-        self.stats = {"device": 0, "host": 0, "general": 0}
+        self.stats = {"device": 0, "host": 0, "general": 0, "jpeg": 0}
 
     def _buffers(self, n: int):
         """-> (PNG buffer, pinned text, device table, pinned table) for an n-byte text, or None when they cannot all be
@@ -342,6 +353,13 @@ class DeviceChecks:
         settle (HostParse) gets the host path's answer from png_of_payload itself.  -> (DevicePng or bytes, PngInfo)."""
         import torch
         text = payload_text(image)
+        if text.startswith(JPEG_B64):
+            # a JPEG body: the host b64decode and Huffman decode, off the event loop; the device check is PNG-only
+            self.stats["jpeg"] += 1
+            png, info = await asyncio.get_running_loop().run_in_executor(None, png_of_payload, image)
+            if isinstance(info, JpegInfo):
+                self.pool.hold(info.coefs)
+            return png, info
         try:
             raw = text.encode("ascii")                  # b64decode refuses a str with other characters the same way
         except UnicodeEncodeError as exc:
@@ -659,7 +677,8 @@ class GpuFrames:
 
     def add(self, items: Sequence[dict]):
         """A PNG kept on this device (DevicePng, stored blocks) is decoded where it lies; any other is uploaded (a
-        PngGeneral's filtered stream, to usdu_png_decode_general_u8)."""
+        PngGeneral's filtered stream, to usdu_png_decode_general_u8; a JpegInfo's coefficients, to
+        usdu_jpeg_decode_u8)."""
         import torch
         if not items:
             return

@@ -6,7 +6,8 @@ The routes and the job store live on ComfyUI's server event loop, as in the refe
 reaches them with `run_coroutine_threadsafe`.  A route handler never decodes pixels: it validates each posted PNG on the
 host (`parse_png`, which refuses what PIL's open().convert("RGB") refuses) and keeps the raw bytes, the segment table of
 the filtered stream inside them and the tile's metadata.  A palette, 1/2/4/16-bit or interlaced PNG, which parse_png
-refuses, is validated and inflated by `parse_png_general` instead, and its filtered stream kept.  The master uploads each
+refuses, is validated and inflated by `parse_png_general` instead, and its filtered stream kept; a baseline JPEG is
+parsed and Huffman-decoded by `parse_jpeg` (csrc/usdu_jpeg.cpp), and its coefficients kept.  The master uploads each
 drained batch of tiles and decodes it on a side stream (csrc/usdu_png_decode.cu) while it waits for more, and
 composites all kept worker tiles in the reference's order with the existing blend kernels.
 
@@ -21,6 +22,7 @@ Differences from the reference (INTEGRATION.md, "A master for HTTP workers"):
 from __future__ import annotations
 
 import asyncio
+import io
 import json
 import os
 import struct
@@ -262,6 +264,59 @@ def parse_png_any(data: bytes):
         return parse_png(data)
     except UnsupportedPng:
         return parse_png_general(data)
+
+
+# --------------------------------------------------------------------------------------
+# baseline JPEG (csrc/usdu_jpeg.cpp on the host, csrc/usdu_jpeg_decode.cu on the device)
+# --------------------------------------------------------------------------------------
+JPEG_SOI = b"\xff\xd8\xff"
+
+
+class JpegInfo:
+    """A baseline JPEG the library takes (usdu_jpeg_parse): `info` its JPEG_INFO_WORDS words, `quant` int32 [3, 64]
+    tables, `coefs` the int16 coefficient blocks of its Huffman decode."""
+    __slots__ = ("W", "H", "info", "quant", "coefs", "__weakref__")
+
+    def __init__(self, info, quant, coefs):
+        from . import _native as nat
+        self.info, self.quant, self.coefs = info, quant, coefs
+        self.W, self.H = int(info[nat.JI_W]), int(info[nat.JI_H])
+
+
+def _pil_header_opens(data: bytes, W: int, H: int) -> bool:
+    """PIL's own verdict on the header: Image.open parses the markers up to SOS in Python (APPn contents, Exif for the
+    DPI, an MPF index) before libjpeg sees the file, and raises on some it cannot read.  Reads no pixels."""
+    try:
+        from PIL import Image
+        with warnings.catch_warnings():
+            warnings.simplefilter("ignore")
+            with Image.open(io.BytesIO(data)) as im:
+                return im.format == "JPEG" and im.size == (W, H)
+    except Exception:
+        return False
+
+
+def parse_jpeg(data: bytes) -> JpegInfo:
+    """The marker parse and Huffman decode of a baseline JPEG, or ValueError with the reason for every file it does not
+    take: the library's (include/usdu_b200.h, usdu_jpeg_parse), or a header PIL's Image.open refuses."""
+    from . import _native as nat
+    info, quant = nat.jpeg_parse(data)
+    if not _pil_header_opens(data, int(info[nat.JI_W]), int(info[nat.JI_H])):
+        raise ValueError("JPEG: PIL does not open its header")
+    coefs = np.empty(int(info[nat.JI_BLOCKS]) * 64, np.int16)
+    nat.jpeg_decode_coefs(data, coefs)
+    return JpegInfo(info, quant, coefs)
+
+
+def parse_image_any(data: bytes):
+    """parse_jpeg for bytes that start with the JPEG SOI, else parse_png_any.  A JPEG parse_jpeg refuses gets
+    parse_png_any's answer, the refusal any JPEG had before this path existed.  -> JpegInfo, PngInfo or PngGeneral."""
+    if data[:3] == JPEG_SOI:
+        try:
+            return parse_jpeg(data)
+        except ValueError:
+            pass
+    return parse_png_any(data)
 
 
 class _IdatStream:
@@ -562,7 +617,7 @@ def parse_tiles_from_form(data) -> List[dict]:
             raise ValueError(f"Missing tile data for index {i}")
         raw = field.file.read()
         try:
-            info = parse_png_any(raw)
+            info = parse_image_any(raw)
         except Exception as e:
             raise ValueError(f"Invalid image data for tile {i}: {e}")
         try:
@@ -632,8 +687,8 @@ def make_handlers(store: JobStore):
                     if job is not None:
                         job.queue.put_nowait({"worker_id": worker_id, "is_last": True, "tiles": []})
                         return web.json_response({"status": "success"})
-            try:
-                tiles = parse_tiles_from_form(data)
+            try:               # the PNG inflate and the JPEG Huffman decode run off the server loop
+                tiles = await asyncio.get_running_loop().run_in_executor(None, parse_tiles_from_form, data)
             except ValueError as e:
                 return _error(str(e), 400)
             async with store.lock:
@@ -667,7 +722,7 @@ def make_handlers(store: JobStore):
                 int(data.get("image_idx"))
                 img = data["full_image"].file.read()
                 try:
-                    parse_png_any(img)
+                    await asyncio.get_running_loop().run_in_executor(None, parse_image_any, img)
                 except ValueError as e:
                     return _error(e, 500)
             elif not is_last:
@@ -802,14 +857,50 @@ class PngDecoder:
         self._keep_alive = []
 
     def decode(self, items: Sequence[Tuple[object, bytes, int]], dst) -> int:
-        """items: (PngInfo or PngGeneral, PNG bytes, byte offset of the frame's [H, W, 3] u8 output in the device tensor
-        `dst`).  The 8-bit frames go to usdu_png_decode_u8, the others to usdu_png_decode_general_u8, on the side
-        stream.  -> launches made."""
+        """items: (PngInfo, PngGeneral or JpegInfo, the posted bytes, byte offset of the frame's [H, W, 3] u8 output in
+        the device tensor `dst`).  The 8-bit PNGs go to usdu_png_decode_u8, the other PNGs to
+        usdu_png_decode_general_u8, the JPEGs to usdu_jpeg_decode_u8, on the side stream.  -> launches made."""
         general = [it for it in items if isinstance(it[0], PngGeneral)]
-        fast = [it for it in items if not isinstance(it[0], PngGeneral)]
+        jpeg = [it for it in items if isinstance(it[0], JpegInfo)]
+        fast = [it for it in items if not isinstance(it[0], (PngGeneral, JpegInfo))]
         self._decode_fast(fast, dst)
         self.decode_general([(info, off) for info, _, off in general], dst)
-        return int(bool(fast)) + int(bool(general))
+        self.decode_jpeg([(info, off) for info, _, off in jpeg], dst)
+        return int(bool(fast)) + int(bool(general)) + int(bool(jpeg))
+
+    def decode_jpeg(self, items: Sequence[Tuple[JpegInfo, int]], dst):
+        """items: (JpegInfo, byte offset of the frame's output in `dst`): each frame's quantisation tables and
+        coefficients uploaded through pinned memory, one usdu_jpeg_decode_u8 launch over all of them."""
+        import torch
+        from . import _native as nat
+        if not items:
+            return
+        blobs, descs, pos, ctas = [], [], 0, 0
+        for info, off in items:
+            w = info.info
+            q_at, c_at = pos, pos + info.quant.nbytes
+            blobs += [(q_at, info.quant.view(np.uint8).reshape(-1)), (c_at, info.coefs.view(np.uint8))]
+            pos = (c_at + info.coefs.nbytes + 15) // 16 * 16
+            descs.append([c_at, q_at, info.W, info.H, w[nat.JI_COMPONENTS], w[nat.JI_H0], w[nat.JI_V0],
+                          w[nat.JI_COLOUR], w[nat.JI_MCUX], w[nat.JI_MCUY], off, ctas, 0, 0, 0, 0])
+            ctas += int(w[nat.JI_MCUY]) * ((info.W + nat.JPEG_TILE_W - 1) // nat.JPEG_TILE_W)
+        tabs = np.asarray(descs, np.int64).reshape(-1)
+        host = torch.empty(pos + tabs.nbytes, dtype=torch.uint8, pin_memory=True)
+        h = host.numpy()
+        for at, blob in blobs:
+            h[at: at + blob.size] = blob
+        h[pos:] = tabs.view(np.uint8)
+        with torch.cuda.device(self.device), torch.cuda.stream(self.side):
+            dev = torch.empty(host.numel(), dtype=torch.uint8, device=self.device)
+            e_up, e0, e1 = (torch.cuda.Event(enable_timing=True) for _ in range(3))
+            e_up.record(self.side)
+            dev.copy_(host, non_blocking=True)
+            e0.record(self.side)
+            nat.jpeg_decode_u8(dev.data_ptr(), dev.data_ptr() + pos, len(descs), ctas, dst.data_ptr(),
+                               self.side.cuda_stream)
+            e1.record(self.side)
+        self._events.append((e_up, e0, e1))
+        self._keep_alive.append((host, dev, dst))
 
     def decode_general(self, items: Sequence[Tuple[PngGeneral, int]], dst):
         """items: (PngGeneral, byte offset of the frame's output in `dst`): each frame's R and palette uploaded through

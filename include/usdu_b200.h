@@ -35,7 +35,7 @@ extern "C" {
 #pragma GCC visibility push(default) /* the library itself is built with -fvisibility=hidden */
 #endif
 
-#define USDU_ABI_VERSION 18
+#define USDU_ABI_VERSION 19
 
 typedef enum usdu_status {
     USDU_OK = 0,
@@ -346,6 +346,56 @@ int usdu_png_decode_warps(int max_row_bytes);
 #define USDU_PNG_GENERAL_DESC_WORDS 16
 int usdu_png_decode_general_u8(const uint8_t* src_dev, const int64_t* descs_dev, int n, int max_row_bytes,
                                uint8_t* dst_dev, void* stream);
+
+/* Baseline JPEGs at the masters' routes, decoded as PIL's open().convert("RGB") with libjpeg-turbo's defaults (islow
+ * IDCT, fancy upsampling, table-driven YCbCr->RGB).  The entropy decode is serial and runs on the host
+ * (csrc/usdu_jpeg.cpp); dequantisation, IDCT, upsampling and colour conversion run on the device.
+ * Taken: SOF0/SOF1, 8-bit, one scan of every component, 1 component, or 3 with the first at h, v in {1, 2} and the
+ * others 1x1; sides up to 65,500 (libjpeg's JPEG_MAX_DIMENSION); any DQT/DHT tables, DRI with RST0..7 in sequence,
+ * APPn/COM skipped, except the APPn segments PIL's Python header parse raises on (short "JFIF" APP0, "Adobe" APP14 and
+ * "ICC_PROFILE" APP2, a cut "Photoshop 3.0" 8BIM resource) and "MPF" APP2 (an MPO).  Everything else, and every file
+ * whose markers, Huffman codes, MCU count, restart markers or EOI are not exactly right, fails with USDU_ERR_INVALID
+ * and the reason in usdu_last_error (also where libjpeg would only warn).
+ * usdu_jpeg_parse: data[n] (host) -> info (USDU_JPEG_INFO_WORDS int64, the USDU_JI_* words) and quant (3 * 64 int32:
+ *   each component's quantisation table in natural order, zeros for absent components).
+ * usdu_jpeg_decode_coefs: the Huffman decode of the same file into coefs (host, n_words = 64 * info[USDU_JI_BLOCKS]
+ *   int16): per component in order, a raster of 8x8 blocks over the MCU-padded component (bw x bh blocks, bw = MCUX *
+ *   h, bh = MCUY * v, h = v = 1 for components after the first and for a 1-component file), each block's 64
+ *   coefficients in natural (row-major) order, not dequantised. */
+#define USDU_JPEG_INFO_WORDS 16
+#define USDU_JI_W 0
+#define USDU_JI_H 1
+#define USDU_JI_COMPONENTS 2 /* 1 or 3 */
+#define USDU_JI_H0 3         /* sampling of the first component (1 for a 1-component file) */
+#define USDU_JI_V0 4
+#define USDU_JI_COLOUR 5     /* USDU_JPEG_GREY, _YCC or _RGB, as libjpeg's default_decompress_parms decides */
+#define USDU_JI_RESTART 6    /* restart interval in MCUs, 0 without DRI */
+#define USDU_JI_MCUX 7       /* MCUs across and down */
+#define USDU_JI_MCUY 8
+#define USDU_JI_BLOCKS 9     /* coefficient blocks of all components */
+#define USDU_JI_SCAN 10      /* offset of the first entropy-coded byte */
+#define USDU_JPEG_GREY 0
+#define USDU_JPEG_YCC 1
+#define USDU_JPEG_RGB 2
+int usdu_jpeg_parse(const uint8_t* data, int64_t n, int64_t* info, int32_t* quant);
+int usdu_jpeg_decode_coefs(const uint8_t* data, int64_t n, int16_t* coefs, int64_t n_words);
+
+/* usdu_jpeg_decode_u8: n frames, one launch of n_ctas CTAs; a CTA decodes one tile of a frame, one MCU row by
+ * USDU_JPEG_TILE_W pixels, into the frame's [H, W, 3] u8 output.
+ * descs_dev: n descriptors of USDU_JPEG_DESC_WORDS int64: offset in src_dev of the frame's coefficients (the layout of
+ *   usdu_jpeg_decode_coefs, 16-byte aligned), offset in src_dev of its 3 * 64 int32 quantisation tables (4-byte
+ *   aligned), W, H, components, h0, v0, colour, MCUX, MCUY (the USDU_JI_* words), byte offset of the frame's output in
+ *   dst_dev, index of the frame's first CTA (0 for the first frame, then the running sum of MCUY * ceil(W /
+ *   USDU_JPEG_TILE_W)), then 0s.  n_ctas is the sum over all frames.
+ * The stages restate libjpeg-turbo's: dequantisation and the islow IDCT as its x86 SIMD code computes them (16-bit
+ * dequantised coefficients, its 16-bit sums and saturating packs, which equal jidctint.c's results wherever no
+ * intermediate leaves 16 bits); h2v1, h1v2 and h2v2 fancy upsampling with its rounding biases and edge rows and
+ * columns (replication when a subsampled chroma row is at most 2 samples wide, as jdsample.c chooses); ycc_rgb_convert's
+ * fixed-point tables, or no conversion for RGB; a grey frame replicated into the 3 channels. */
+#define USDU_JPEG_DESC_WORDS 16
+#define USDU_JPEG_TILE_W 128
+int usdu_jpeg_decode_u8(const uint8_t* src_dev, const int64_t* descs_dev, int n, int64_t n_ctas, uint8_t* dst_dev,
+                        void* stream);
 
 /* HTTP tile worker transport (upscale/worker_comms.py:30-34): each u8 RGB frame [H, W, 3] as the PNG Pillow writes with
  * compress_level=0, byte for byte.  At level 0 Pillow's file is a framing that depends on the shape alone, filled with

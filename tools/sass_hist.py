@@ -15,7 +15,8 @@ kern, hist = None, {}
 for line in txt.splitlines():
     m = re.search(r"Function : (\S+)", line)
     if m:
-        kern = subprocess.run(["c++filt", m.group(1)], capture_output=True, text=True).stdout.strip().split("(")[0]
+        # cut the parameter list only: "usdu::(anonymous namespace)::k(...)" keeps its namespace
+        kern = subprocess.run(["c++filt", m.group(1)], capture_output=True, text=True).stdout.strip().rsplit("(", 1)[0]
         hist[kern] = collections.Counter()
         continue
     m = re.search(r"/\*[0-9a-f]{4}\*/\s+(?:@!?U?P\d+\s+)?([A-Z][A-Z0-9_]*)((?:\.[A-Z0-9_]+)*)", line)
